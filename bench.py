@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — kriged grid points / second of the B200 backend='cuda' execute() path.
+"""bench.py — kriged grid points / second of the backend='cuda' execute() path on an H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--configs cfg1,cfg3,...|none]
+                    [--dump-outputs DIR]
 
 Headline workload (BASELINE.json configs[1], SURVEY.md §8d cfg2): OrdinaryKriging 2-D, N=5000 random-scatter
 data (seed 1002), 1000x1000 grid, exponential variogram [1.0, 300, 0.05], fp64 (DMMA kernel).
@@ -29,6 +30,10 @@ N=100000, 4000x4000) — each run on the N GPUs of this launch (their named GPU 
 same way, with 4096+16-point parity against the CPU oracle checked in the run. A failed check of the HEADLINE aborts the
 bench (no number without parity); a side config that fails its check, or raises, stays in the line flagged
 `"invalid"` / `"error"` instead of taking the measured headline down with it.
+
+--dump-outputs DIR writes what the last timed headline step computed, (z, sigma^2) of every grid point of the fixed
+1000x1000 grid in fp64 (16 MB), as DIR/zvalues.npy and DIR/sigmasq.npy; the inputs are seeded, so two builds run with
+the same arguments can be compared output for output.
 """
 import os
 import sys
@@ -67,7 +72,7 @@ CONFIGS = {
     "cfg4": dict(cls="UK", dim=2, n=10000, seed=1004, grid=(2000, 2000), box=(1000.0, 1000.0), model="exponential",
                  params=[1.0, 300.0, 0.05], dtype="float32", named_gpus=4,
                  text="UniversalKriging 2D regional-linear drift, N=10000 data, 2000x2000 grid, fp32 device math "
-                      "(tcgen05 3xTF32) (BASELINE configs[3])"),
+                      "(wgmma 3xTF32) (BASELINE configs[3])"),
     "cfg5": dict(cls="OK", dim=2, n=100000, seed=1005, grid=(4000, 4000), box=(1000.0, 1000.0), model="exponential",
                  params=[1.0, 50.0, 0.05], dtype="float64", k=64, named_gpus=8,
                  text="OrdinaryKriging 2D moving window n_closest_points=64, N=100000 data, 4000x4000 grid "
@@ -353,9 +358,10 @@ def oracle_parity(ctx, cfg, model, xyz, val, axes, z_loc, ss_loc, first, count, 
     return out
 
 
-def bench_config(ctx, name, steps, warmup, e2e_steps, weak=False, dtype=None, parity=True, fatal_parity=False):
+def bench_config(ctx, name, steps, warmup, e2e_steps, weak=False, dtype=None, parity=True, fatal_parity=False, dump=None):
     """Time one BASELINE config on the ranks of this launch. Device-resident step (factor + krige this rank's
-    contiguous slice, outputs left in HBM) and end-to-end step (public API, host buffers). Max over ranks."""
+    contiguous slice, outputs left in HBM) and end-to-end step (public API, host buffers). Max over ranks.
+    dump: a dict that receives, on rank 0, (z, sigma^2) of the whole grid from the last timed device step."""
     import pykrige_b200 as pk  # noqa: F401
     from pykrige_b200 import multigpu
     torch, dist = ctx.torch, ctx.dist
@@ -415,6 +421,15 @@ def bench_config(ctx, name, steps, warmup, e2e_steps, weak=False, dtype=None, pa
         step_dev()
     h.reset_counters()
     ms_dev = timed(ctx, step_dev, steps)
+    if dump is not None:
+        zs = d_out[:2 * count].view(2, count).cpu().numpy()
+        parts = [(first, zs)]
+        if ctx.world > 1:
+            parts = [None] * ctx.world
+            dist.all_gather_object(parts, (first, zs))
+        parts.sort(key=lambda p: p[0])
+        dump["zvalues"] = np.concatenate([p[1][0] for p in parts])
+        dump["sigmasq"] = np.concatenate([p[1][1] for p in parts])
     tm = h.timings()
     launches = torch.tensor([tm["launches"]], dtype=torch.float64, device=ctx.dev)
     if ctx.world > 1:
@@ -455,7 +470,7 @@ def roofline_for(cfg, res, peaks):
     alg, exe = flop_per_point(cfg), executed_flop_per_point(cfg)
     if cfg["dtype"] == "float32":
         peak, src, kern = peaks["tf32"], "torch.matmul fp32 8192^3 with TF32 allowed (cuBLAS), this run", \
-            "solve_kernel_tf32 (tcgen05.mma kind::tf32, 3xTF32 split: 3 tensor MACs per algorithmic MAC)"
+            "solve_kernel_tf32 (wgmma .tf32, 3xTF32 split: 3 tensor MACs per algorithmic MAC)"
         exe *= 3.0
     else:
         peak, src = peaks["fp64"], "torch.matmul fp64 8192^3 (cuBLAS DGEMM), best of 3, this run"
@@ -467,20 +482,6 @@ def roofline_for(cfg, res, peaks):
             "peak_source": src, "algorithmic_flop_per_point": alg, "executed_flop_per_point": exe,
             "points_per_launch": pts / res["kernel_launches_per_step"],
             "avg_launch_ms": res["kernel_ms_rank0"] / res["kernel_launches_per_step"]}
-
-
-def static_traffic():
-    """DRAM bytes per launch of the headline kernel from the committed ncu --set full capture (NOT measured in
-    this run: ncu cannot run inside a timed bench)."""
-    for rel in ("profiles/r02/solve_kernel_summary.json", "profiles/solve_kernel_summary.json"):
-        p = os.path.join(ROOT, rel)
-        if os.path.exists(p):
-            try:
-                d = json.load(open(p))
-                return d.get("dram_bytes_per_launch"), "static: %s (ncu --set full, 1e6-point launch)" % rel
-            except Exception:  # noqa: BLE001
-                pass
-    return None, "no committed ncu capture"
 
 
 def run_ours(args):
@@ -516,7 +517,12 @@ def run_ours(args):
     # ---- headline: cfg2, fixed 1000x1000 grid split over the ranks (strong scaling) ----
     sampler = ClockSampler(local)
     sampler.start()
-    head, cfg2 = bench_config(ctx, "cfg2", args.steps, args.warmup, args.steps, parity=True, fatal_parity=True)
+    dump = {} if args.dump_outputs else None
+    head, cfg2 = bench_config(ctx, "cfg2", args.steps, args.warmup, args.steps, parity=True, fatal_parity=True, dump=dump)
+    if dump is not None and ctx.rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in dump.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), arr.astype(np.float64))
     sampler.stop_flag = True
     sampler.join(timeout=2.0)
 
@@ -541,8 +547,8 @@ def run_ours(args):
                 res, cfg = bench_config(ctx, "cfg2", osteps, owarm, min(2, osteps), dtype=dt)
             except Exception as e:  # noqa: BLE001
                 res = {"workload": CONFIGS["cfg2"]["text"], "dtype": dt, "error": "%s: %s" % (type(e).__name__, e)}
-            res["kernel"] = ("solve_kernel_i8: tcgen05.mma kind::i8, %s error-free slices, exact int32 accumulation in "
-                             "TMEM, exact int64 recombination" % ("6 (41-bit)" if dt == "float64x" else "4 (27-bit)"))
+            res["kernel"] = ("solve_kernel_i8: wgmma .s32.s8.s8, %s error-free slices, exact int32 accumulation in "
+                             "registers, exact int64 recombination" % ("6 (41-bit)" if dt == "float64x" else "4 (27-bit)"))
             f64x[dt] = res
     weak = None
     if ctx.world > 1:
@@ -554,9 +560,6 @@ def run_ours(args):
 
     if ctx.rank == 0:
         roof = roofline_for(cfg2, head, peaks)
-        traffic, tsrc = static_traffic()
-        roof["traffic"] = traffic
-        roof["traffic_source"] = tsrc
         roof["note"] = ("frac = algorithmic 2(N+1)^2 flop/point (the reference's inverse GEMV, SURVEY.md 8d) over the measured "
                         "DGEMM rate; the kernel executes the covariance-form triangular product (about half of that), so frac "
                         "can exceed 1; frac_executed is the utilisation of the fp64 tensor pipe")
@@ -607,6 +610,8 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--configs", default="cfg1,cfg3,cfg4,cfg5",
                     help="other BASELINE configs to run after the headline (comma list, or 'none')")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write (z, sigma^2) of the last timed headline step as DIR/zvalues.npy, DIR/sigmasq.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)

@@ -1,5 +1,5 @@
 /*
- * krige_b200.h — C ABI of libkrige_b200.so, the B200-native kriging execute() backend.
+ * krige_b200.h — C ABI of libkrige_b200.so, the H100-native kriging execute() backend.
  *
  * This is the drop-in boundary for PyKrige's `execute(..., backend='cuda')`.
  * It replaces, one level higher (coordinates in, not dense a/bd matrices), the
@@ -57,9 +57,9 @@ extern "C" {
 
 /* ---- arithmetic of the big contraction ---------------------------------- */
 #define KB200_F64 0
-#define KB200_F32 1   /* factorisation stays fp64; contraction in 3xTF32 on tcgen05 (fp32-class accuracy) */
+#define KB200_F32 1   /* factorisation stays fp64; contraction in 3xTF32 on wgmma (fp32-class accuracy) */
 #define KB200_F64X 2  /* fp64-class contraction on the INT8 tensor cores: error-free slicing into 6 signed slices (41 bits),
-                         exact int32 accumulation (tcgen05 kind::i8), exact int64 recombination; agrees with KB200_F64
+                         exact int32 accumulation (wgmma .s32.s8.s8), exact int64 recombination; agrees with KB200_F64
                          to ~1e-10 */
 #define KB200_F64X5 3 /* the same with 5 slices (34 bits, 15 instead of 21 MMAs per k-step) */
 #define KB200_F64X4 4 /* the same with 4 slices (27 bits, 10 MMAs per k-step): between float32 and float64 */
@@ -85,7 +85,7 @@ int  kb200_version(void);
  * (ok.py:626-648,663; uk.py:861-920,935).
  *
  *  dim            2 or 3
- *  dtype          KB200_F64 (DMMA) / KB200_F32 (tcgen05 3xTF32) / KB200_F64X, KB200_F64X5, KB200_F64X4 (tcgen05 INT8 slices)
+ *  dtype          KB200_F64 (DMMA) / KB200_F32 (wgmma 3xTF32) / KB200_F64X, KB200_F64X5, KB200_F64X4 (wgmma INT8 slices)
  *  n              number of data points
  *  x,y,z          host, length n, ORIGINAL (un-adjusted) coordinates; z may be NULL when dim==2
  *  values         host, length n (self.Z / self.VALUES)

@@ -1,14 +1,12 @@
-"""Builds oracle/_ref/: the reference's OWN native twins of the hot path, compiled from the sources where
-they lie under /root/reference (read-only; no reference source is copied into the repo):
+"""Builds oracle/_ref/: the reference's OWN native twins of the hot path, compiled from the reference's sources at
+REF_LIB (read-only; no reference source is copied into the repo):
 
-    /root/reference/src/pykrige/lib/cok.pyx               _c_exec_loop (cok.pyx:14-96),
-                                                          _c_exec_loop_moving_window (cok.pyx:98-193)
-    /root/reference/src/pykrige/lib/variogram_models.pyx  the C variogram table (variogram_models.pyx:5-21)
+    lib/cok.pyx               _c_exec_loop (cok.pyx:14-96), _c_exec_loop_moving_window (cok.pyx:98-193)
+    lib/variogram_models.pyx  the C variogram table (variogram_models.pyx:5-21)
 
-TEST INFRASTRUCTURE ONLY (same rule as oracle/krige_oracle.py): used by tests/ to check the numpy
-restatement and the CUDA path against the reference's compiled code, and by bench.py's cpu_baseline leg.
-Outputs go only into oracle/_ref/ (git-ignored, NOT gpurun-ignored: the .so files travel to the GPU box,
-where /root/reference does not exist):
+TEST INFRASTRUCTURE ONLY (same rule as oracle/krige_oracle.py): tests/golden/make_golden.py runs the twins and stores
+their outputs in tests/golden/ref_twins.npz, which the tests compare against, so no test needs them; bench.py's
+cpu_baseline leg also times them when they are built. Outputs go only into oracle/_ref/ (git-ignored):
 
     oracle/_ref/build/*.c                       Cython-generated C, deleted again after compilation
     oracle/_ref/pykrige/lib/{cok,variogram_models}.<abi>.so
@@ -17,7 +15,7 @@ where /root/reference does not exist):
 The package has to be importable as `pykrige.lib.*`: Cython bakes the qualified name of the cimported
 module (`from .variogram_models cimport get_variogram_model`, cok.pyx:11) into the extension.
 
-    python oracle/build_ref.py          # no-op when /root/reference is absent (GPU box: prebuilt files)
+    python oracle/build_ref.py          # no-op when the reference's sources are absent
 """
 import os
 import subprocess

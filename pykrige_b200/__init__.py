@@ -1,8 +1,8 @@
-"""pykrige_b200 — B200-native ``backend='cuda'`` kriging ``execute()`` path.
+"""pykrige_b200 — H100-native ``backend='cuda'`` kriging ``execute()`` path.
 
 Keeps the class API of GeoStat-Framework/PyKrige (OrdinaryKriging, UniversalKriging,
 OrdinaryKriging3D, UniversalKriging3D) and its variogram_models plug-in surface; the
-kriging system is assembled, factored and solved by hand-written sm_100a CUDA kernels
+kriging system is assembled, factored and solved by hand-written sm_90a CUDA kernels
 behind a C ABI (include/krige_b200.h, pykrige_b200/csrc). No CPU fallback.
 """
 from . import variogram_models  # noqa: F401

@@ -1,7 +1,7 @@
 """ctypes binding of libkrige_b200.so (include/krige_b200.h).
 
 This is the thin shim named in BASELINE.json's north_star: Python host code calling
-hand-written sm_100a CUDA through a C ABI. There is no CPU fallback — if the shared
+hand-written sm_90a CUDA through a C ABI. There is no CPU fallback — if the shared
 library is missing, or no CUDA device is present, the backend raises.
 """
 import ctypes

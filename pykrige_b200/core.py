@@ -1,4 +1,4 @@
-"""Host-side helpers of the B200 kriging backend (numpy/scipy, constructor-time only).
+"""Host-side helpers of the H100 kriging backend (numpy/scipy, constructor-time only).
 
 Mirrors the behaviour of the reference's ``src/pykrige/core.py`` for the pieces the
 kriging classes need around ``execute()``; none of this is on the hot path:

@@ -14,8 +14,8 @@
 
 #define KB_VERSION 2000
 static const int64_t KB_STAGE_PTS = 1 << 20;   // prediction points per staged output chunk (2 x 8 MB through pinned memory)
-#define KB_TILE_COST_32 0.532     // one round of 32-point tiles relative to one round of 64-point tiles (fp64 kernel, N=5000:
-#define KB_TILE_COST_16 0.301     // 7.34 / 3.91 / 2.21 ms per round; scripts/tile_timing.py, profiles/r02/tile_width_timing_run21.log)
+#define KB_TILE_COST_32 0.540     // one round of 32-point tiles relative to one round of 64-point tiles (fp64 kernel, N=5000,
+#define KB_TILE_COST_16 0.309     // one H100 at 400 W: 8.11 / 4.38 / 2.51 ms per round; scripts/tile_timing.py)
 static const int64_t KB_STAGE_MIN = 1 << 18;   // below this the outputs go straight to the caller's buffers
 
 struct Src {
@@ -72,7 +72,7 @@ struct kb200_ctx {
     DevBuf wC, wW, wT, wF, wRaw, wFlag;
     // execute workspace
     DevBuf wPart, wAux, wPts, wOut, wAxes, wDrift, wScratch;
-    int num_sms = 148;
+    int num_sms = 132;
     // device-evaluated drift terms (kb200_set_device_drift): configuration + the count used by the described problem
     DeviceDrift dd{};
     DevBuf wWells, wExt;
@@ -126,7 +126,7 @@ extern "C" int kb200_create(kb200_handle* out, int device) {
     for (auto& ev : h->ev) if (cudaEventCreate(&ev) != cudaSuccess) { delete h; return KB200_ECUDA; }
     if (kbk_factor_init() != cudaSuccess || kbk_solve_init() != cudaSuccess || kbk_solve_tf32_init() != cudaSuccess ||
         kbk_solve_i8_init() != cudaSuccess || kbk_ev_init() != cudaSuccess || kbk_pinv_init() != cudaSuccess) { delete h; return KB200_ECUDA; }
-    if (cudaDeviceGetAttribute(&h->num_sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || h->num_sms < 1) h->num_sms = 148;
+    if (cudaDeviceGetAttribute(&h->num_sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || h->num_sms < 1) h->num_sms = 132;
     *out = h;
     return KB200_OK;
 }
@@ -656,7 +656,7 @@ static int launch_solve(kb200_ctx* h, const Src& s, double* d_z, double* d_ss, i
 }
 
 // Relative cost of one round of the fp64 kernel with 64 / 32 / 16-point tiles (a tile streams all of W once whatever its
-// width; the DMMA work is proportional to the width). Measured at N=5000 (profiles/r02/tile_width_timing_*.log).
+// width; the DMMA work is proportional to the width), at N=5000 (scripts/tile_timing.py).
 static double tile_cost(int tp) { return tp == 64 ? 1.0 : (tp == 32 ? KB_TILE_COST_32 : KB_TILE_COST_16); }
 
 // NOTE: the summation order per point does not depend on the tile width, on how the points are sharded or chunked, or on

@@ -1,4 +1,4 @@
-// common.cuh — shared device helpers for libkrige_b200 (sm_100a).
+// common.cuh — shared device helpers for libkrige_b200 (sm_90a).
 //
 // Semantics follow the reference (cited per function); the code is written from
 // scratch for the GPU.
@@ -205,7 +205,7 @@ __device__ __forceinline__ void kb_load_point(const PointSource& ps, const Aniso
     kb_adjust<DIM>(an, rx, ry, rz, x, y, z);
 }
 
-// ---- mma.sync m8n8k4 f64 (DMMA): the fp64 tensor path on sm_100a ------------
+// ---- mma.sync m8n8k4 f64 (DMMA): the fp64 tensor path on sm_90a -------------
 // A 8x4 row: lane holds A[lane>>2][lane&3]; B 4x8 col: lane holds B[lane&3][lane>>2];
 // C 8x8: lane holds C[lane>>2][2*(lane&3) + {0,1}].
 __device__ __forceinline__ void kb_dmma(double& c0, double& c1, double a, double b) {
@@ -214,9 +214,10 @@ __device__ __forceinline__ void kb_dmma(double& c0, double& c1, double a, double
 }
 
 // ---- L2 cache policies for the bulk copies of the solve kernels ----------------------------------------------
-// The factor tile stream (W) is read by every CTA for every point tile: keep it resident (evict_last). The per-CTA
-// RHS scratch ring is private, far larger than L2 in total (148 x n x tile bytes) and dead after one tile:
-// evict_first, so that it does not push W out (ncu, round 2: L2 hit rate 18-27 % without the hints).
+// The factor tile stream (W) is read by every CTA for every point tile: keep what L2 holds of it (evict_last; DESIGN.md §2
+// has the measurement on H100, where W outgrows L2 above N ~ 3500). The per-CTA
+// RHS scratch ring is private, far larger than L2 in total (one ring per SM, n x tile bytes each) and dead after one
+// tile: evict_first, so that it does not push W out.
 __device__ __forceinline__ uint64_t kb_policy_evict_last() {
     uint64_t p;
     asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;\n" : "=l"(p));
@@ -232,6 +233,26 @@ __device__ __forceinline__ void kb_bulk_g2s_hint(void* dst, const void* src, uin
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;\n"
                  :: "r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src), "r"(bytes),
                     "r"((uint32_t)__cvta_generic_to_shared(bar)), "l"(policy) : "memory");
+}
+
+// ---- warpgroup MMA (wgmma, sm_90a) helpers for the tensor-core solve kernels ---------------------------------
+// Shared-memory matrix descriptor, K-major, no swizzle ("interleave" layout): 8-row x 16-byte core matrices,
+// lbo = byte stride between the two k-adjacent core matrices one instruction reads, sbo = byte stride between
+// 8-row groups. Bits 0-13 start address >> 4, 16-29 lbo >> 4, 32-45 sbo >> 4, layout type (62-63) 0.
+__device__ __forceinline__ uint64_t kb_wgmma_desc(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
+    return (uint64_t)((smem_addr >> 4) & 0x3fffu) | ((uint64_t)((lbo >> 4) & 0x3fffu) << 16) |
+           ((uint64_t)((sbo >> 4) & 0x3fffu) << 32);
+}
+__device__ __forceinline__ void kb_wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void kb_wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void kb_wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" :: "n"(N) : "memory"); }
+// keeps the compiler from moving accesses of an accumulator register across a wgmma wait
+__device__ __forceinline__ void kb_reg_fence(float& r) { asm volatile("" : "+f"(r) :: "memory"); }
+__device__ __forceinline__ void kb_reg_fence(uint32_t& r) { asm volatile("" : "+r"(r) :: "memory"); }
+// named barrier over the first `threads` threads of the block (id 0 is __syncthreads)
+__device__ __forceinline__ void kb_named_sync(int id, int threads) {
+    asm volatile("bar.sync %0, %1;\n" :: "r"(id), "r"(threads) : "memory");
 }
 
 #define KB_CUDA_OK(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) return _e; } while (0)

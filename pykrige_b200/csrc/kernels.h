@@ -180,7 +180,7 @@ cudaError_t kbk_solve_init();   // opt-in shared memory attributes
 cudaError_t kbk_solve_pt(int dim, const SolvePtParams& p, int grid, int tile_points /* 64 | 32 | 16 */, cudaStream_t st);
 size_t      kbk_solve_pt_scratch_doubles(int n, int grid);
 
-// fp32 path (solve_tf32.cu): tcgen05.mma kind::tf32, 3xTF32 split, TMEM accumulators
+// fp32 path (solve_tf32.cu): wgmma .tf32, 3xTF32 split, fp32 accumulators in registers
 cudaError_t kbk_solve_tf32_init();
 cudaError_t kbk_solve_tf32(int dim, const SolvePtParams& p, int grid, cudaStream_t st);
 cudaError_t kbk_pack_tf32(const double* W, int ld, int n, int n_pad, int na, const double* Uz, const PackMap& pm,

@@ -12,7 +12,7 @@
 //   solve_kernel_pt   (K3 v3, the product path) persistent CTAs, one CTA = 64 points x all rows of W, RHS column
 //                     block generated once per tile, W/RHS tiles streamed by cp.async.bulk + mbarrier, fused
 //                     finalize. See the comment above the kernel.
-// The tcgen05 variants live in solve_tf32.cu (dtype float32) and solve_i8.cu (dtype float64x).
+// The wgmma variants live in solve_tf32.cu (dtype float32) and solve_i8.cu (dtype float64x).
 #include "common.cuh"
 #include "kernels.h"
 #include <cstdlib>
@@ -71,7 +71,7 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 
 // NT = n-tiles (of 8 points) per point tile: 8 (64 points) is the default. Narrower tiles (NT = 4, 2: 32 / 16 points) are used by
 // the host for the TAIL of a launch: the points left over after the last full round of 64-point tiles would keep only a few of
-// the 148 persistent CTAs busy for a whole tile time (1953 tiles on 148 SMs = 13.2 rounds: 4.9 of 102 ms at 125 000 points per
+// the persistent CTAs (one per SM) busy for a whole tile time (1953 tiles on 132 SMs = 14.8 rounds at 125 000 points per
 // GPU); as narrow tiles they spread over all SMs and a tile costs little more than streaming W once. The per-point arithmetic
 // does not depend on NT (tests/test_parity_gpu.py::test_tile_width_is_invisible).
 template <int DIM, int MODEL, int NT>

@@ -1,40 +1,39 @@
 // solve_i8.cu — K3 for dtype = KB200_F64X / F64X5 / F64X4: fp64-class accuracy of q_j = ||W c_j||^2 (DESIGN.md §3)
-// on the INT8 path of the 5th-generation tensor cores (tcgen05.mma kind::i8, exact int32 accumulation in TMEM).
+// on the INT8 path of the Hopper tensor cores (wgmma.mma_async .s32.s8.s8, exact int32 accumulation in registers).
 //
 // Error-free slicing (the "Ozaki scheme"): every row of W and every RHS column is scaled by a power of two
 // into (-1, 1) and cut into S signed slices of 6+7+...+7 bits (S = 6: 41 bits, 5: 34 bits, 4: 27 bits),
 //      x = 2^e * sum_s slice_s * 2^(-6-7s),   |slice_s| <= 64,
 // so that  W_rk c_k = 2^(ew_r + ec_j) * sum_{s,t} w_s c_t 2^(-12-7(s+t)).  All slice products with the
-// same d = s + t are summed EXACTLY in one int32 TMEM accumulator (|sum| <= n * (d+1) * 64^2 < 2^31 for
+// same d = s + t are summed EXACTLY in one int32 accumulator (|sum| <= n * (d+1) * 64^2 < 2^31 for
 // n <= 32512); pairs with d >= S are dropped (relative 2^-(7S+6) per term). The S accumulators are combined
 // exactly in int64 in the epilogue and converted to fp64 once. S = 6 agrees with the fp64 DMMA kernel to ~1e-10
-// (tests) at several times its rate; fewer slices trade bits for MMAs (S(S+1)/2 per k-stage: 21 / 15 / 10) and
-// operand bytes; dtype='float64' keeps the DMMA kernel as the default.
+// (tests); fewer slices trade bits for MMAs (S(S+1)/2 per k-stage: 21 / 15 / 10) and operand bytes;
+// dtype='float64' keeps the DMMA kernel as the default.
 //
-// Orientation as in solve_tf32.cu: D[point][W row], M = 128 points (TMEM lanes), N = BN W rows per row block
-// with S * BN <= 512 TMEM columns (BN = 80 / 96 / 128: the RHS slices are re-read once per row block, so fewer
-// slices also mean fewer re-reads), K = 32 per MMA; operands in the canonical no-swizzle K-major UMMA layout
+// Orientation as in solve_tf32.cu: D[point][W row], M = 64 points per CTA tile, N = BN W rows per row block, split
+// between two consumer warpgroups (BN / 2 rows each, S * BN / 4 int32 accumulators per thread: BN = 48 / 64 / 64 for
+// S = 6 / 5 / 4 keeps them in registers), K = 32 per MMA; operands in the no-swizzle K-major core-matrix layout
 // (8-row x 16-byte core matrices, k-chunks 128 B apart, 8-row groups 256 B apart), one stage = 32 k = one MMA
 // k-step. The variogram model is a run-time switch here (phase G is < 10 % of the kernel), so that the slice
 // count and the dimension are the only template parameters.
 #include "common.cuh"
 #include "kernels.h"
 
-#define I8_THREADS 512
-#define I8_GEN_THREADS 256                 // warps 8..15: two generator threads per prediction point
-#define I8_TM 128
+#define I8_CONS_THREADS 256                // warps 0-7: two consumer warpgroups
+#define I8_GEN_THREADS 192                 // warps 9-14: three generator threads per prediction point
+#define I8_THREADS (I8_CONS_THREADS + 32 + I8_GEN_THREADS)
+#define I8_TM 64
 #define I8_BK 32
-#define I8_C_SLICE (I8_TM * I8_BK)            // 4 KB
+#define I8_C_SLICE (I8_TM * I8_BK)            // 2 KB
 
 template <int S> struct I8Cfg {
-    static constexpr int BN = (S == 6) ? 80 : (S == 5) ? 96 : 128;     // S * BN <= 512 TMEM columns, BN % 16 == 0
-    static constexpr int STAGES = (S == 4) ? 6 : 5;
+    static constexpr int BN = (S == 6) ? 48 : 64;      // BN / 2 is a valid wgmma N; S * BN / 4 accumulators per thread
+    static constexpr int STAGES = 6;
     static constexpr int W_SLICE = BN * I8_BK;
     static constexpr int W_BYTES = S * W_SLICE;
     static constexpr int C_BYTES = S * I8_C_SLICE;
     static constexpr int STAGE_BYTES = W_BYTES + C_BYTES;
-    // D = S32 (bits 4-5 = 2), A = B = signed 8 bit (bits 7-9, 10-12 = 1), K-major, N = BN, M = 128
-    static constexpr uint32_t IDESC = (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(I8_TM >> 4) << 24);
 };
 
 __device__ __forceinline__ uint32_t i8_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -58,24 +57,25 @@ __device__ __forceinline__ void i8_mbar_wait(uint64_t* bar, uint32_t parity) {
     }
     __trap();
 }
-__device__ __forceinline__ void i8_bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
-                 :: "r"(i8_smem_u32(dst)), "l"(src), "r"(bytes), "r"(i8_smem_u32(bar)) : "memory");
-}
-// K-major, no swizzle: LBO (k-chunk stride) = 128 B, SBO (8-row group stride) = 256 B, version 1
-__device__ __forceinline__ uint64_t i8_desc(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr >> 4) & 0x3fffu) | ((uint64_t)(128u >> 4) << 16) | ((uint64_t)(256u >> 4) << 32) |
-           (1ull << 46);
-}
-__device__ __forceinline__ void i8_mma(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\t"
-                 "setp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}\n"
-                 :: "r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void i8_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n"
-                 :: "r"(i8_smem_u32(bar)) : "memory");
+// K-major, no swizzle: LBO (k-chunk stride) = 128 B, SBO (8-row group stride) = 256 B
+__device__ __forceinline__ uint64_t i8_desc(uint32_t smem_addr) { return kb_wgmma_desc(smem_addr, 128u, 256u); }
+// d[64 points x R*2 W rows] (+)= A[64 x 32] B[R*2 x 32]^T in int32; scale_d = 0 overwrites d
+template <int R>
+__device__ __forceinline__ void i8_mma(uint32_t (&d)[R], uint64_t da, uint64_t db, uint32_t scale_d) {
+    static_assert(R == 12 || R == 16, "wgmma N = 24 or 32");
+    if constexpr (R == 12) {
+        asm volatile("{\n\t.reg .pred p;\n\t"
+                     "setp.ne.b32 p, %14, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n24k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11}, %12, %13, p;\n\t}\n"
+                     : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11])
+                     : "l"(da), "l"(db), "r"(scale_d) : "memory");
+    } else {
+        asm volatile("{\n\t.reg .pred p;\n\t"
+                     "setp.ne.b32 p, %18, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n\t}\n"
+                     : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+                     : "l"(da), "l"(db), "r"(scale_d) : "memory");
+    }
 }
 
 // S signed 7-bit digits of y = x * 2^-e (|y| < 1): x = 2^e * sum_s out[s] * 2^(-6-7s) + O(2^(e-7S)), out[s] in [-64, 64].
@@ -142,7 +142,7 @@ __global__ void __launch_bounds__(256) i8_rowscale_kernel(const double* __restri
     }
 }
 
-// tile (row block J, k stage t): S slices x (BN rows x 32 k) int8 in UMMA layout
+// tile (row block J, k stage t): S slices x (BN rows x 32 k) int8 in the wgmma operand layout
 template <int S>
 __global__ void __launch_bounds__(256) i8_pack_kernel(const double* __restrict__ W, int ld, int n, int n_pad, int na,
                                                        const double* __restrict__ Uz, const int* __restrict__ rowexp,
@@ -179,27 +179,26 @@ __device__ __forceinline__ double i8_cov_rhs(const VgParams& v, double d) {
     }
 }
 
-// Warp roles (512 threads): warp 0 lane 0 = bulk-copy producer, warp 1 lane 0 = MMA issuer, warp 2 = TMEM allocator,
-// warps 4-7 = epilogue (thread = TMEM lane = prediction point), warps 8-15 = RHS generators (two threads per point,
-// alternating k-stages: the fp64 sqrt/exp chains are latency-bound, eight warps keep the pipe fed; twelve gave +2 % at
-// S = 4 and -8 % at S = 6 through register spills).
+// Warp roles (480 threads): warps 0-7 = two consumer warpgroups (wgmma, epilogue, finalize), warp 8 lane 0 = bulk-copy
+// producer, warps 9-14 = RHS generators (three threads per point, interleaved k-stages: the fp64 sqrt/exp chains are
+// latency-bound).
 // The generators work one point tile AHEAD of the tensor pipe: they evaluate and slice the RHS column block of
 // tile i+1 into the other half of the double-buffered scratch ring while the MMAs of tile i run (the fp64 pipe
 // and the tensor pipe do not compete); gfull / gempty mbarriers hand the buffers over.
 template <int S, int DIM>
 __global__ void __launch_bounds__(I8_THREADS, 1) solve_kernel_i8(const __grid_constant__ SolvePtParams P) {
     typedef I8Cfg<S> C;
+    constexpr int NH = C::BN / 2;                        // W rows per consumer warpgroup
+    constexpr int R = NH / 2;                            // int32 accumulators per thread and slice sum
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     unsigned char* stage_base = smem_raw;                                                    // STAGES * STAGE_BYTES
-    double* auxs = reinterpret_cast<double*>(smem_raw + (size_t)C::STAGES * C::STAGE_BYTES);  // KB_MAXAUX * 128
-    int* pexp = reinterpret_cast<int*>(auxs + KB_MAXAUX * I8_TM);                            // 2 x 128 point exponents
+    double* auxs = reinterpret_cast<double*>(smem_raw + (size_t)C::STAGES * C::STAGE_BYTES);  // KB_MAXAUX * 64
+    double* qpart = auxs + KB_MAXAUX * I8_TM;                                                // 2 warpgroups x 64 points
+    int* pexp = reinterpret_cast<int*>(qpart + 2 * I8_TM);                                   // 2 x 64 point exponents
     uint64_t* full = reinterpret_cast<uint64_t*>(pexp + 2 * I8_TM);                          // STAGES
     uint64_t* empty = full + C::STAGES;
-    uint64_t* tfull = empty + C::STAGES;                                                     // 1
-    uint64_t* tempty = tfull + 1;                                                            // 1
-    uint64_t* gfull = tempty + 1;                                                            // 2
+    uint64_t* gfull = empty + C::STAGES;                                                     // 2
     uint64_t* gempty = gfull + 2;                                                            // 2
-    uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(gempty + 2);
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int nk = (P.n + I8_BK - 1) / I8_BK;
@@ -211,26 +210,17 @@ __global__ void __launch_bounds__(I8_THREADS, 1) solve_kernel_i8(const __grid_co
     const int model = P.vg.model;
 
     if (tid == 0) {
-        for (int s = 0; s < C::STAGES; ++s) { i8_mbar_init(&full[s], 1); i8_mbar_init(&empty[s], 1); }
-        i8_mbar_init(tfull, 1); i8_mbar_init(tempty, 4);
-        for (int b = 0; b < 2; ++b) { i8_mbar_init(&gfull[b], I8_GEN_THREADS); i8_mbar_init(&gempty[b], 4); }
+        for (int s = 0; s < C::STAGES; ++s) { i8_mbar_init(&full[s], 1); i8_mbar_init(&empty[s], 2); }
+        for (int b = 0; b < 2; ++b) { i8_mbar_init(&gfull[b], I8_GEN_THREADS); i8_mbar_init(&gempty[b], 1); }
         asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
         asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n"
-                     :: "r"(i8_smem_u32(tmem_base_smem)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-    const uint32_t tmem_base = *tmem_base_smem;
 
-    if (warp >= 8) {
-        // ---------------- generators: RHS column block -> S int8 slices per value, UMMA layout ----------------
-        const int pl = (tid - 8 * 32) & (I8_TM - 1);       // 0..127: point within the tile
-        const int ks = (tid - 8 * 32) >> 7;                // 0..1: k-stage parity handled by this thread
+    if (warp >= 9) {
+        // ---------------- generators: RHS column block -> S int8 slices per value, wgmma layout ----------------
+        const int pl = (tid - 9 * 32) & (I8_TM - 1);       // 0..63: point within the tile
+        const int ks = (tid - 9 * 32) / I8_TM;             // 0..2: k-stage residue handled by this thread
         uint32_t it = 0;
         for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
             const int b = (int)(it & 1);
@@ -288,7 +278,7 @@ __global__ void __launch_bounds__(I8_THREADS, 1) solve_kernel_i8(const __grid_co
             asm volatile("fence.proxy.async.global;\n" ::: "memory");
             i8_mbar_arrive(&gfull[b]);
         }
-    } else if (warp == 0) {
+    } else if (warp == 8) {
         // ---------------- producer: W tiles + RHS tiles -> smem ring ----------------
         if (lane == 0) {
             const uint64_t pol_w = kb_policy_evict_last(), pol_c = kb_policy_evict_first();
@@ -311,103 +301,87 @@ __global__ void __launch_bounds__(I8_THREADS, 1) solve_kernel_i8(const __grid_co
                 }
             }
         }
-    } else if (warp == 1) {
-        // ---------------- MMA issuer ----------------
-        if (lane == 0) {
-            uint32_t gg = 0, gb = 0;
-            for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-                for (int J = 0; J < nrb; ++J, ++gb) {
-                    const int kt = i8_ktiles(J, P.n, nk, C::BN);
-                    i8_mbar_wait(tempty, (uint32_t)((gb & 1) ^ 1));
-                    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-                    for (int t = 0; t < kt; ++t, ++gg) {
-                        const int s = gg % C::STAGES;
-                        i8_mbar_wait(&full[s], (uint32_t)((gg / C::STAGES) & 1));
-                        asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-                        const uint32_t wb = i8_smem_u32(stage_base + (size_t)s * C::STAGE_BYTES);
-                        const uint32_t cb = wb + C::W_BYTES;
-#pragma unroll
-                        for (int d = 0; d < S; ++d) {
-#pragma unroll
-                            for (int sw = 0; sw <= d; ++sw) {
-                                const int sc = d - sw;                                     // slice of c
-                                const uint32_t acc = (t == 0 && sw == 0) ? 0u : 1u;
-                                i8_mma(tmem_base + (uint32_t)d * C::BN, i8_desc(cb + sc * I8_C_SLICE),
-                                       i8_desc(wb + sw * C::W_SLICE), C::IDESC, acc);
-                            }
-                        }
-                        i8_commit(&empty[s]);
-                    }
-                    i8_commit(tfull);
-                }
-            }
-        }
-    } else if (warp >= 4) {
-        // ---------------- epilogue: thread = TMEM lane = prediction point ----------------
-        const int pl = (warp & 3) * 32 + lane;
-        const uint32_t t_addr = tmem_base + (((uint32_t)(warp & 3) * 32u) << 16);
-        uint32_t gb = 0, it = 0;
+    } else {
+        // ---------------- consumers: warpgroup h owns W rows [NH h, NH h + NH) of every row block ----------------
+        // accumulator element i = 4 j + 2 hh + e of (warp w of the group, lane): point 16 w + lane / 4 + 8 hh,
+        // row NH h + 8 j + 2 (lane % 4) + e
+        const int h = warp >> 2, wtid = tid & 127;
+        const int p0 = (warp & 3) * 16 + (lane >> 2);       // points p0 and p0 + 8
+        const uint32_t hoff = (uint32_t)h * (NH / 8) * 256u;
+        uint32_t gg = 0, it = 0;
         for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
             const int b = (int)(it & 1);
             i8_mbar_wait(&gfull[b], (it >> 1) & 1);            // acquire the generators' pexp[b]
-            const double pscale = scalbn(1.0, pexp[b * I8_TM + pl] - 7 * (S - 1));
-            double q = 0.0;
-            for (int J = 0; J < nrb; ++J, ++gb) {
-                i8_mbar_wait(tfull, (uint32_t)(gb & 1));
-                asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-#pragma unroll 1
-                for (int ch = 0; ch < C::BN / 16; ++ch) {
-                    // exact recombination: V = sum_d acc_d * 2^(7 (S-1-d)) fits in int64 (|acc_d| < 2^30, d = 0 has one
-                    // slice pair: < 2^27 * 2^35)
-                    long long V[16];
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) V[j] = 0;
+            double pscale[2];
+            for (int hh = 0; hh < 2; ++hh) pscale[hh] = scalbn(1.0, pexp[b * I8_TM + p0 + 8 * hh] - 7 * (S - 1));
+            double q[2] = {0.0, 0.0};
+            for (int J = 0; J < nrb; ++J) {
+                const int kt = i8_ktiles(J, P.n, nk, C::BN);
+                uint32_t acc[S][R];
+                for (int t = 0; t < kt; ++t, ++gg) {
+                    const int s = gg % C::STAGES;
+                    i8_mbar_wait(&full[s], (uint32_t)((gg / C::STAGES) & 1));
+                    kb_wgmma_fence();
+                    const uint32_t wb = i8_smem_u32(stage_base + (size_t)s * C::STAGE_BYTES) + hoff;
+                    const uint32_t cb = i8_smem_u32(stage_base + (size_t)s * C::STAGE_BYTES) + C::W_BYTES;
 #pragma unroll
                     for (int d = 0; d < S; ++d) {
-                        uint32_t u[16];
-                        asm volatile(
-                            "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-                            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-                            : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7]),
-                              "=r"(u[8]), "=r"(u[9]), "=r"(u[10]), "=r"(u[11]), "=r"(u[12]), "=r"(u[13]), "=r"(u[14]), "=r"(u[15])
-                            : "r"(t_addr + (uint32_t)d * C::BN + (uint32_t)ch * 16u));
-                        asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
 #pragma unroll
-                        for (int j = 0; j < 16; ++j) V[j] = V[j] * 128 + (long long)(int)u[j];
-                    }
-                    const int r0 = J * C::BN + ch * 16;
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const int r = r0 + j;
-                        if (r < P.n + P.na) {
-                            const double x = (double)V[j] * (__ldg(P.rowscale + r) * pscale);
-                            if (r < P.n) q += x * x;
-                            else auxs[(r - P.n) * I8_TM + pl] = x;
+                        for (int sw = 0; sw <= d; ++sw) {
+                            const int sc = d - sw;                                     // slice of c
+                            i8_mma(acc[d], i8_desc(cb + sc * I8_C_SLICE), i8_desc(wb + sw * C::W_SLICE),
+                                   (t == 0 && sw == 0) ? 0u : 1u);
                         }
                     }
+                    kb_wgmma_commit();
+                    kb_wgmma_wait<1>();                  // the previous stage has been read: hand it back
+                    if (t > 0 && wtid == 0) i8_mbar_arrive(&empty[(gg - 1) % C::STAGES]);
                 }
-                asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-                __syncwarp();
-                if (lane == 0) i8_mbar_arrive(tempty);
+                kb_wgmma_wait<0>();
+                if (wtid == 0) i8_mbar_arrive(&empty[(gg - 1) % C::STAGES]);
+#pragma unroll
+                for (int d = 0; d < S; ++d)
+#pragma unroll
+                    for (int i = 0; i < R; ++i) kb_reg_fence(acc[d][i]);
+                const int rb = J * C::BN + h * NH + 2 * (lane & 3);
+#pragma unroll
+                for (int i = 0; i < R; ++i) {
+                    const int r = rb + 8 * (i >> 2) + (i & 1), hh = (i >> 1) & 1;
+                    if (r < P.n + P.na) {
+                        // exact recombination: V = sum_d acc_d * 2^(7 (S-1-d)) fits in int64 (|acc_d| < 2^30, d = 0 has
+                        // one slice pair: < 2^27 * 2^35)
+                        long long V = 0;
+#pragma unroll
+                        for (int d = 0; d < S; ++d) V = V * 128 + (long long)(int)acc[d][i];
+                        const double x = (double)V * (__ldg(P.rowscale + r) * pscale[hh]);
+                        if (r < P.n) q[hh] += x * x;
+                        else auxs[(r - P.n) * I8_TM + p0 + 8 * hh] = x;
+                    }
+                }
             }
+            // the four lanes of a point hold interleaved rows; then the two warpgroups
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+                q[hh] += __shfl_xor_sync(0xffffffffu, q[hh], 1);
+                q[hh] += __shfl_xor_sync(0xffffffffu, q[hh], 2);
+                if ((lane & 3) == 0) qpart[h * I8_TM + p0 + 8 * hh] = q[hh];
+            }
+            kb_named_sync(1, I8_CONS_THREADS);
             // ---------------- phase F: finalize (DESIGN.md §3), thread = point ----------------
-            const long long pj = tile * I8_TM + pl;
-            if (pj < P.m) kb_finalize_point<DIM, double>(P, pj, q, auxs + pl, I8_TM);
-            __syncwarp();
-            if (lane == 0) i8_mbar_arrive(&gempty[b]);       // scratch half b and pexp[b] may be rewritten
+            if (tid < I8_TM) {
+                const long long pj = tile * I8_TM + tid;
+                if (pj < P.m) kb_finalize_point<DIM, double>(P, pj, qpart[tid] + qpart[I8_TM + tid], auxs + tid, I8_TM);
+            }
+            kb_named_sync(1, I8_CONS_THREADS);
+            if (tid == 0) i8_mbar_arrive(&gempty[b]);       // scratch half b and pexp[b] may be rewritten
         }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-    __syncthreads();
-    if (warp == 2) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" :: "r"(tmem_base), "r"(512u) : "memory");
     }
 }
 
 // ---- host side ---------------------------------------------------------------------------------------
 template <int S> static size_t i8_smem_s() {
-    return (size_t)I8Cfg<S>::STAGES * I8Cfg<S>::STAGE_BYTES + (size_t)KB_MAXAUX * I8_TM * sizeof(double) + 2 * I8_TM * sizeof(int) +
-           (2 * I8Cfg<S>::STAGES + 6) * sizeof(uint64_t) + 64;
+    return (size_t)I8Cfg<S>::STAGES * I8Cfg<S>::STAGE_BYTES + (size_t)KB_MAXAUX * I8_TM * sizeof(double) +
+           2 * I8_TM * sizeof(double) + 2 * I8_TM * sizeof(int) + (2 * I8Cfg<S>::STAGES + 4) * sizeof(uint64_t) + 64;
 }
 static int i8_bn(int S) { return S == 6 ? I8Cfg<6>::BN : S == 5 ? I8Cfg<5>::BN : I8Cfg<4>::BN; }
 bool kbk_i8_valid_slices(int S) { return S >= 4 && S <= 6; }

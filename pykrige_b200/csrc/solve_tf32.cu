@@ -1,31 +1,30 @@
 // solve_tf32.cu — K3 for dtype = KB200_F32: the same covariance-form contraction q_j = ||W c_j||^2
-// (DESIGN.md §3) on the 5th-generation tensor cores: tcgen05.mma kind::tf32 with the accumulator in
-// TMEM. fp32 accuracy comes from the 3xTF32 split  W = Wh + Wl, c = ch + cl (each part exactly
-// representable in TF32):  W c ~= Wh ch + Wh cl + Wl ch  accumulated in fp32 (measured error of
-// sigma^2: 3e-6 relative, tolerance for fp32 is 1e-2).
+// (DESIGN.md §3) on the Hopper tensor cores: wgmma.mma_async m64n128k8 .tf32 with fp32 accumulators in
+// registers. fp32 accuracy comes from the 3xTF32 split  W = Wh + Wl, c = ch + cl (each part exactly
+// representable in TF32):  W c ~= Wh ch + Wh cl + Wl ch  accumulated in fp32 (tolerance for fp32 is 1e-2).
 //
-// Orientation: D[point][row of W] so that one TMEM lane = one prediction point; the epilogue then
-// needs no cross-lane reduction (each thread squares-and-adds its own 256 columns).
-//   A operand (M = 128 points)  : RHS tile, K-major, from the per-CTA scratch ring (generated once per
-//                                 point tile by all warps, fp32 sqrt/exp on fp64 coordinate differences)
-//   B operand (N = 256 W rows)  : W tile, K-major, packed by pack_tf32_kernel
-//   both in the canonical no-swizzle ("interleaved") UMMA layout: 8-row x 16-byte core matrices,
-//   k-chunks 128 B apart (LBO), 8-row groups 512 B apart (SBO); one stage = 16 k = 2 MMA k-steps.
-// Roles: warp 0 = bulk-copy producer (cp.async.bulk + mbarrier), warp 1 = MMA issuer (one lane),
-// warp 2 = TMEM allocator, warps 4..7 = epilogue (tcgen05.ld) + per-point finalize.
-// Two 256-column accumulators alternate between row blocks so the epilogue of block I overlaps the
-// MMAs of block I+1.
+// Orientation: D[point][row of W], M = 64 points per CTA tile, N = 256 W rows per row block, split between two
+// consumer warpgroups (128 rows = 64 fp32 accumulators per thread each). Each thread squares-and-adds its own
+// accumulators; the four lanes sharing a point and the two warpgroups are summed once per point tile.
+//   A operand (64 points)  : RHS tile, K-major, from the per-CTA scratch ring (generated once per point tile
+//                            by the generator warps, fp32 sqrt/exp on fp64 coordinate differences)
+//   B operand (256 W rows) : W tile, K-major, packed by pack_tf32_kernel
+//   both in the no-swizzle K-major core-matrix layout: 8-row x 16-byte core matrices, k-chunks 128 B apart (LBO),
+//   8-row groups 512 B apart (SBO); one stage = 16 k = 2 wgmma k-steps.
+// Roles (480 threads): warps 0-7 = two consumer warpgroups (wgmma + epilogue + per-point finalize), warp 8 lane 0 =
+// bulk-copy producer (cp.async.bulk + mbarrier), warps 9-14 = RHS generators (three threads per point).
 #include "common.cuh"
 #include "kernels.h"
 
 #define TF_STAGES 4
-#define TF_THREADS 512
-#define TF_GEN_THREADS 256              // warps 8..15: two generator threads per prediction point
-#define TF_TM 128                  // points per CTA tile (UMMA M)
-#define TF_BN KB_BM                // W rows per row block (UMMA N) = 256
+#define TF_CONS_THREADS 256                 // warps 0-7: two consumer warpgroups
+#define TF_GEN_THREADS 192                  // warps 9-14: three generator threads per prediction point
+#define TF_THREADS (TF_CONS_THREADS + 32 + TF_GEN_THREADS)
+#define TF_TM 64                   // points per CTA tile (wgmma M)
+#define TF_BN KB_BM                // W rows per row block = 256 (two wgmma N = 128 halves)
 #define TF_BK KB_BK                // k per stage = 16
 #define TF_W_BYTES (TF_BN * TF_BK * 4 * 2)     // hi + lo = 32 KB
-#define TF_C_BYTES (TF_TM * TF_BK * 4 * 2)     // hi + lo = 16 KB
+#define TF_C_BYTES (TF_TM * TF_BK * 4 * 2)     // hi + lo = 8 KB
 #define TF_STAGE_BYTES (TF_W_BYTES + TF_C_BYTES)
 
 __device__ __forceinline__ uint32_t tf_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -49,37 +48,34 @@ __device__ __forceinline__ void tf_mbar_wait(uint64_t* bar, uint32_t parity) {
     }
     __trap();     // a lost arrival traps instead of hanging the GPU
 }
-__device__ __forceinline__ void tf_bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
-                 :: "r"(tf_smem_u32(dst)), "l"(src), "r"(bytes), "r"(tf_smem_u32(bar)) : "memory");
-}
 __device__ __forceinline__ float tf32_round(float x) {
     uint32_t u;
     asm("cvt.rna.tf32.f32 %0, %1;\n" : "=r"(u) : "f"(x));
     return __uint_as_float(u);
 }
-// K-major, no swizzle: start address, LBO (k-chunk stride) = 128 B, SBO (8-row group stride) = 512 B,
-// descriptor version 1 (Blackwell), layout type 0 (cute::UMMA::SmemDescriptor bit layout)
-__device__ __forceinline__ uint64_t tf_desc(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr >> 4) & 0x3fffu) | ((uint64_t)(128u >> 4) << 16) | ((uint64_t)(512u >> 4) << 32) |
-           (1ull << 46);
-}
-// instruction descriptor: D = F32 (bits 4-5 = 1), A = B = TF32 (bits 7-9, 10-12 = 2), K-major A and B,
-// N = 256 (bits 17-22 = N >> 3), M = 128 (bits 24-28 = M >> 4)
-#define TF_IDESC ((1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TF_BN >> 3) << 17) | ((uint32_t)(TF_TM >> 4) << 24))
+__device__ __forceinline__ uint64_t tf_desc(uint32_t smem_addr) { return kb_wgmma_desc(smem_addr, 128u, 512u); }
 
-__device__ __forceinline__ void tf_mma(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t accumulate) {
+// d[64 points x 128 W rows] (+)= A[64 x 8] B[128 x 8]^T; scale_d = 0 overwrites d
+__device__ __forceinline__ void tf_mma(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
     asm volatile("{\n\t.reg .pred p;\n\t"
-                 "setp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n"
-                 :: "r"(tmem_d), "l"(da), "l"(db), "r"(TF_IDESC), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tf_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n"
-                 :: "r"(tf_smem_u32(bar)) : "memory");
+                 "setp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, "
+                 "%22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, "
+                 "%43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+                 "%64, %65, p, 1, 1;\n\t}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+                   "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+                   "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+                   "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+                   "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+                   "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(da), "l"(db), "r"(scale_d) : "memory");
 }
 
-// ---- pack: W (fp64, row-major lower triangle) + dual rows -> TF32 hi/lo tiles in UMMA layout --------
+// ---- pack: W (fp64, row-major lower triangle) + dual rows -> TF32 hi/lo tiles in wgmma layout -------
 // tile (row block I, k stage t): 8192 floats = [hi 4096][lo 4096];
 //   element (r, k) of a part at float offset (r/8)*128 + (k/4)*32 + (r%8)*4 + (k%4)
 __global__ void __launch_bounds__(256) pack_tf32_kernel(const double* __restrict__ W, int ld, int n, int n_pad, int na,
@@ -123,15 +119,13 @@ __device__ __forceinline__ float tf_cov_rhs(const VgParams& v, double dd) {
 template <int DIM, int MODEL>
 __global__ void __launch_bounds__(TF_THREADS, 1) solve_kernel_tf32(const __grid_constant__ SolvePtParams P) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    unsigned char* stage_base = smem_raw;                                            // TF_STAGES * 48 KB
-    float* auxs = reinterpret_cast<float*>(smem_raw + (size_t)TF_STAGES * TF_STAGE_BYTES);   // KB_MAXAUX * 128
-    uint64_t* full = reinterpret_cast<uint64_t*>(auxs + KB_MAXAUX * TF_TM);          // TF_STAGES
+    unsigned char* stage_base = smem_raw;                                            // TF_STAGES * 40 KB
+    float* auxs = reinterpret_cast<float*>(smem_raw + (size_t)TF_STAGES * TF_STAGE_BYTES);   // KB_MAXAUX * 64
+    double* qpart = reinterpret_cast<double*>(auxs + KB_MAXAUX * TF_TM);            // 2 warpgroups x 64 points
+    uint64_t* full = reinterpret_cast<uint64_t*>(qpart + 2 * TF_TM);                // TF_STAGES
     uint64_t* empty = full + TF_STAGES;                                              // TF_STAGES
-    uint64_t* tfull = empty + TF_STAGES;                                             // 2
-    uint64_t* tempty = tfull + 2;                                                    // 2
-    uint64_t* gfull = tempty + 2;                                                    // 2
+    uint64_t* gfull = empty + TF_STAGES;                                             // 2
     uint64_t* gempty = gfull + 2;                                                    // 2
-    uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(gempty + 2);
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int nk = (P.n + TF_BK - 1) / TF_BK;
@@ -141,29 +135,19 @@ __global__ void __launch_bounds__(TF_THREADS, 1) solve_kernel_tf32(const __grid_
     const long long ntiles = (P.m + TF_TM - 1) / TF_TM;
 
     if (tid == 0) {
-        for (int s = 0; s < TF_STAGES; ++s) { tf_mbar_init(&full[s], 1); tf_mbar_init(&empty[s], 1); }
-        for (int b = 0; b < 2; ++b) { tf_mbar_init(&tfull[b], 1); tf_mbar_init(&tempty[b], 4); }
-        for (int b = 0; b < 2; ++b) { tf_mbar_init(&gfull[b], TF_GEN_THREADS); tf_mbar_init(&gempty[b], 4); }
+        for (int s = 0; s < TF_STAGES; ++s) { tf_mbar_init(&full[s], 1); tf_mbar_init(&empty[s], 2); }
+        for (int b = 0; b < 2; ++b) { tf_mbar_init(&gfull[b], TF_GEN_THREADS); tf_mbar_init(&gempty[b], 1); }
         asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
         asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n"
-                     :: "r"(tf_smem_u32(tmem_base_smem)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-    const uint32_t tmem_base = *tmem_base_smem;
 
-    // Warp roles (512 threads): warp 0 lane 0 = bulk-copy producer, warp 1 lane 0 = MMA issuer, warp 2 = TMEM allocator,
-    // warps 4-7 = epilogue, warps 8-15 = RHS generators working ONE POINT TILE AHEAD of the tensor pipe into the other
-    // half of a double-buffered scratch ring (gfull / gempty mbarriers), as in solve_i8.cu.
-    if (warp >= 8) {
-        const int gt_ = tid - 8 * 32;
+    // The generators work ONE POINT TILE AHEAD of the tensor pipe into the other half of a double-buffered scratch
+    // ring (gfull / gempty mbarriers), as in solve_i8.cu.
+    if (warp >= 9) {
+        const int gt_ = tid - 9 * 32;
         const int pl = gt_ & (TF_TM - 1);
-        const int ks = gt_ >> 7;                           // 0..1
+        const int ks = gt_ / TF_TM;                        // 0..2
         uint32_t it = 0;
         for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
             const int b = (int)(it & 1);
@@ -199,7 +183,7 @@ __global__ void __launch_bounds__(TF_THREADS, 1) solve_kernel_tf32(const __grid_
             asm volatile("fence.proxy.async.global;\n" ::: "memory");
             tf_mbar_arrive(&gfull[b]);
         }
-    } else if (warp == 0) {
+    } else if (warp == 8) {
         if (lane == 0) {
             const uint64_t pol_w = kb_policy_evict_last(), pol_c = kb_policy_evict_first();
             uint32_t gg = 0, it = 0;
@@ -221,97 +205,79 @@ __global__ void __launch_bounds__(TF_THREADS, 1) solve_kernel_tf32(const __grid_
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            uint32_t gg = 0, gb = 0;
-            for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-                for (int I = 0; I < P.nrb; ++I, ++gb) {
-                    const int kt = P.pm.ktiles[I];
-                    const int buf = gb & 1;
-                    tf_mbar_wait(&tempty[buf], (uint32_t)(((gb >> 1) & 1) ^ 1));
-                    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-                    const uint32_t d_tmem = tmem_base + (uint32_t)buf * TF_BN;
-                    for (int t = 0; t < kt; ++t, ++gg) {
-                        const int s = gg % TF_STAGES;
-                        tf_mbar_wait(&full[s], (uint32_t)((gg / TF_STAGES) & 1));
-                        asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-                        const uint32_t wb = tf_smem_u32(stage_base + (size_t)s * TF_STAGE_BYTES);
-                        const uint32_t w_hi = wb, w_lo = wb + TF_W_BYTES / 2;
-                        const uint32_t c_hi = wb + TF_W_BYTES, c_lo = c_hi + TF_C_BYTES / 2;
-#pragma unroll
-                        for (int kstep = 0; kstep < TF_BK / 8; ++kstep) {
-                            const uint32_t ko = (uint32_t)kstep * 256u;          // 2 k-chunks of 128 B
-                            const uint32_t first = (t == 0 && kstep == 0) ? 0u : 1u;
-                            tf_mma(d_tmem, tf_desc(c_hi + ko), tf_desc(w_hi + ko), first);
-                            tf_mma(d_tmem, tf_desc(c_hi + ko), tf_desc(w_lo + ko), 1u);
-                            tf_mma(d_tmem, tf_desc(c_lo + ko), tf_desc(w_hi + ko), 1u);
-                        }
-                        tf_commit(&empty[s]);              // stage free once these MMAs have read it
-                    }
-                    tf_commit(&tfull[buf]);                // accumulator of row block I complete
-                }
-            }
-        }
-    } else if (warp >= 4) {
-        // epilogue: thread = TMEM lane = prediction point
-        const int pl = (warp & 3) * 32 + lane;
-        uint32_t gb = 0, it = 0;
+    } else {
+        // consumers: warpgroup h owns W rows [128 h, 128 h + 128) of every row block. Accumulator element
+        // i = 4 j + 2 hh + e of thread (warp w of the group, lane) is point 16 w + lane / 4 + 8 hh, row
+        // 128 h + 8 j + 2 (lane % 4) + e.
+        const int h = warp >> 2, wtid = tid & 127;
+        const int p0 = (warp & 3) * 16 + (lane >> 2);       // points p0 and p0 + 8
+        const int c0 = h * (TF_BN / 2) + 2 * (lane & 3);
+        const uint32_t hoff = (uint32_t)h * (TF_BN / 2 / 8) * 512u;
+        uint32_t gg = 0, it = 0;
         for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-            double q = 0.0;
-            for (int I = 0; I < P.nrb; ++I, ++gb) {
-                const int buf = gb & 1;
-                tf_mbar_wait(&tfull[buf], (uint32_t)((gb >> 1) & 1));
-                asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-                const uint32_t t_addr = tmem_base + (((uint32_t)(warp & 3) * 32u) << 16) + (uint32_t)buf * TF_BN;
-#pragma unroll 1
-                for (int ch = 0; ch < TF_BN / 32; ++ch) {
-                    uint32_t v[32];
-                    asm volatile(
-                        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-                        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-                          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-                          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                        : "r"(t_addr + (uint32_t)ch * 32u));
-                    asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-                    const int r0 = I * TF_BN + ch * 32;
-                    if (r0 + 31 < P.n) {
+            double q[2] = {0.0, 0.0};
+            for (int I = 0; I < P.nrb; ++I) {
+                const int kt = P.pm.ktiles[I];
+                float acc[64];
+                for (int t = 0; t < kt; ++t, ++gg) {
+                    const int s = gg % TF_STAGES;
+                    tf_mbar_wait(&full[s], (uint32_t)((gg / TF_STAGES) & 1));
+                    kb_wgmma_fence();
+                    const uint32_t wb = tf_smem_u32(stage_base + (size_t)s * TF_STAGE_BYTES);
+                    const uint32_t w_hi = wb + hoff, w_lo = wb + TF_W_BYTES / 2 + hoff;
+                    const uint32_t c_hi = wb + TF_W_BYTES, c_lo = c_hi + TF_C_BYTES / 2;
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) { double x = (double)__uint_as_float(v[j]); q += x * x; }
-                    } else if (r0 < P.n + P.na) {
+                    for (int kstep = 0; kstep < TF_BK / 8; ++kstep) {
+                        const uint32_t ko = (uint32_t)kstep * 256u;          // 2 k-chunks of 128 B
+                        tf_mma(acc, tf_desc(c_hi + ko), tf_desc(w_hi + ko), (t == 0 && kstep == 0) ? 0u : 1u);
+                        tf_mma(acc, tf_desc(c_hi + ko), tf_desc(w_lo + ko), 1u);
+                        tf_mma(acc, tf_desc(c_lo + ko), tf_desc(w_hi + ko), 1u);
+                    }
+                    kb_wgmma_commit();
+                    kb_wgmma_wait<1>();                  // the previous stage has been read: hand it back
+                    if (t > 0 && wtid == 0) tf_mbar_arrive(&empty[(gg - 1) % TF_STAGES]);
+                }
+                kb_wgmma_wait<0>();
+                if (wtid == 0) tf_mbar_arrive(&empty[(gg - 1) % TF_STAGES]);
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            const int r = r0 + j;
-                            float x = __uint_as_float(v[j]);
-                            if (r < P.n) q += (double)x * (double)x;
-                            else if (r < P.n + P.na) auxs[(r - P.n) * TF_TM + pl] = x;
-                        }
+                for (int i = 0; i < 64; ++i) kb_reg_fence(acc[i]);
+                const int rb = I * TF_BN + c0;
+                if (I * TF_BN + (h + 1) * (TF_BN / 2) <= P.n) {
+#pragma unroll
+                    for (int i = 0; i < 64; ++i) { const double x = (double)acc[i]; q[(i >> 1) & 1] += x * x; }
+                } else {
+#pragma unroll
+                    for (int i = 0; i < 64; ++i) {
+                        const int r = rb + 8 * (i >> 2) + (i & 1), hh = (i >> 1) & 1;
+                        const float x = acc[i];
+                        if (r < P.n) q[hh] += (double)x * (double)x;
+                        else if (r < P.n + P.na) auxs[(r - P.n) * TF_TM + p0 + 8 * hh] = x;
                     }
                 }
-                asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-                __syncwarp();
-                if (lane == 0) tf_mbar_arrive(&tempty[buf]);
             }
+            // the four lanes of a point hold interleaved columns; then the two warpgroups
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+                q[hh] += __shfl_xor_sync(0xffffffffu, q[hh], 1);
+                q[hh] += __shfl_xor_sync(0xffffffffu, q[hh], 2);
+                if ((lane & 3) == 0) qpart[h * TF_TM + p0 + 8 * hh] = q[hh];
+            }
+            kb_named_sync(1, TF_CONS_THREADS);
             // ---------------- phase F: finalize (DESIGN.md §3), thread = point ----------------
-            const long long pj = tile * TF_TM + pl;
-            if (pj < P.m) kb_finalize_point<DIM, float>(P, pj, q, auxs + pl, TF_TM);
-            __syncwarp();
-            if (lane == 0) tf_mbar_arrive(&gempty[(int)(it & 1)]);      // this tile's scratch half may be rewritten
+            if (tid < TF_TM) {
+                const long long pj = tile * TF_TM + tid;
+                if (pj < P.m) kb_finalize_point<DIM, float>(P, pj, qpart[tid] + qpart[TF_TM + tid], auxs + tid, TF_TM);
+            }
+            kb_named_sync(1, TF_CONS_THREADS);
+            if (tid == 0) tf_mbar_arrive(&gempty[(int)(it & 1)]);      // this tile's scratch half may be rewritten
         }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-    __syncthreads();
-    if (warp == 2) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" :: "r"(tmem_base), "r"(512u) : "memory");
     }
 }
 
 // ---- host side ---------------------------------------------------------------------------------------
 static size_t tf32_smem() {
-    return (size_t)TF_STAGES * TF_STAGE_BYTES + (size_t)KB_MAXAUX * TF_TM * sizeof(float) +
-           (2 * TF_STAGES + 8) * sizeof(uint64_t) + 64;
+    return (size_t)TF_STAGES * TF_STAGE_BYTES + (size_t)KB_MAXAUX * TF_TM * sizeof(float) + 2 * TF_TM * sizeof(double) +
+           (2 * TF_STAGES + 4) * sizeof(uint64_t) + 64;
 }
 
 size_t kbk_solve_tf32_scratch_bytes(int n, int grid) {

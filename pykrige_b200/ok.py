@@ -1,4 +1,4 @@
-"""OrdinaryKriging (2-D) with the B200 ``backend='cuda'`` execute() path.
+"""OrdinaryKriging (2-D) with the H100 ``backend='cuda'`` execute() path.
 
 API mirror of the reference class (src/pykrige/ok.py:187-1020): same constructor
 arguments, public attributes and ``execute`` signature; ``execute`` runs on the GPU

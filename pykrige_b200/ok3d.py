@@ -1,4 +1,4 @@
-"""OrdinaryKriging3D with the B200 ``backend='cuda'`` execute() path.
+"""OrdinaryKriging3D with the H100 ``backend='cuda'`` execute() path.
 
 API mirror of the reference class (src/pykrige/ok3d.py:198-932).
 """

@@ -1,4 +1,4 @@
-"""UniversalKriging (2-D) with the B200 ``backend='cuda'`` execute() path.
+"""UniversalKriging (2-D) with the H100 ``backend='cuda'`` execute() path.
 
 API mirror of the reference class (src/pykrige/uk.py:220-1328). Regional-linear drift is built
 on the device from the adjusted coordinates. The DATA-side columns of the other drift kinds

@@ -1,4 +1,4 @@
-"""UniversalKriging3D with the B200 ``backend='cuda'`` execute() path.
+"""UniversalKriging3D with the H100 ``backend='cuda'`` execute() path.
 
 API mirror of the reference class (src/pykrige/uk3d.py:215-1146): regional-linear drift (three
 columns X, Y, Z built on the device), specified and functional drift (host-evaluated columns).

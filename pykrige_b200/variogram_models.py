@@ -1,4 +1,4 @@
-"""Variogram plug-in surface of the B200 backend.
+"""Variogram plug-in surface of the H100 backend.
 
 Same call signature as the reference's plug-ins — ``f(m, d) -> gamma(d)`` with ``m`` the
 *stored* parameter list (partial-sill form) — and the same function ``__name__`` strings,

@@ -1,5 +1,5 @@
 """Timings of the constructor-side device kernels and of pseudo_inv=True (SURVEY.md §8f next-2 / next-4) on
-one B200, next to the host (numpy/scipy) route of the same repo on the box's CPU. One JSON line per item.
+one H100, next to the host (numpy/scipy) route of the same repo on the box's CPU. One JSON line per item.
 
     python scripts/bench_ctor.py [ev,stats,pinv] [small]
 """

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """Register / stack / spill report of every kernel (ptxas -v; needs no GPU).
 
-    python scripts/ptxas_report.py > profiles/r02/ptxas_resources_final_build.md
+    python scripts/ptxas_report.py > ptxas_resources.md
 
-Compiles each csrc/*.cu for sm_100a with -Xptxas -v (objects go to a temporary directory) and prints, per kernel family,
+Compiles each csrc/*.cu for sm_90a with -Xptxas -v (objects go to a temporary directory) and prints, per kernel family,
 the range of registers per thread, the stack frame and the spill stores / loads over its template instantiations."""
 import collections
 import os
@@ -14,7 +14,7 @@ import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "pykrige_b200", "csrc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 
 
 def family(mangled):
@@ -44,7 +44,7 @@ def main():
                 m = re.search(r"Used (\d+) registers", ln)
                 if m:
                     cur["regs"] = int(m.group(1))
-    print("# ptxas -v resources of the final build (sm_100a, `scripts/ptxas_report.py`)\n")
+    print("# ptxas -v resources of the build (sm_90a, `scripts/ptxas_report.py`)\n")
     print("| file | kernel family | instantiations | registers / thread | stack frame (B) | spill stores (B) | spill loads (B) |")
     print("|---|---|---|---|---|---|---|")
 

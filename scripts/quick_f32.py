@@ -1,4 +1,4 @@
-"""dtype='float32' (tcgen05 3xTF32) vs float64 at config-2 and config-4 sizes: agreement and solve-kernel rate."""
+"""dtype='float32' (wgmma 3xTF32) vs float64 at config-2 and config-4 sizes: agreement and solve-kernel rate."""
 import os, sys, json
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -22,6 +22,8 @@ Writes
       configurations of tests/cases.py fuzz_config (backend='vectorized'; 'loop' for the moving window).
   tests/golden/ref_ctor.npz : lags/semivariance of core._initialize_variogram_model and delta/sigma/epsilon
       of core._find_statistics for the constructor-side cases of tests/cases.py.
+  tests/golden/ref_twins.npz : (z, sigmasq) of the reference's compiled backend='C' loops (oracle/_ref) on the
+      inputs of the twin tests.
 The O(N^4) constructor statistics of OK3D/UK/UK3D are patched out (SURVEY F5); nothing else of the
 reference is touched.
 """
@@ -278,8 +280,55 @@ def ref_fuzz():
     np.savez_compressed(os.path.join(HERE, "ref_fuzz.npz"), **out)
 
 
+def ref_twins():
+    """(z, sigmasq) of the reference's compiled `_c_exec_loop` / `_c_exec_loop_moving_window` (lib/cok.pyx, built into
+    oracle/_ref by oracle/build_ref.py) on the seeded inputs of the twin tests in tests/test_oracle.py and
+    tests/test_parity_gpu.py, so that those tests compare with the reference without needing it."""
+    sys.path.insert(0, ROOT)
+    from oracle import krige_oracle as ko, ref_native as rn
+    # the twins live in a package also named `pykrige`: set the imported reference aside while they load
+    saved = {k: sys.modules.pop(k) for k in list(sys.modules) if k == "pykrige" or k.startswith("pykrige.")}
+    try:
+        out = _twin_outputs(ko, rn)
+    finally:
+        for k in [k for k in sys.modules if k == "pykrige" or k.startswith("pykrige.")]:
+            del sys.modules[k]
+        sys.modules.update(saved)
+    np.savez_compressed(os.path.join(HERE, "ref_twins.npz"), **out)
+
+
+def _twin_outputs(ko, rn):
+    assert rn.available(), "oracle/_ref is not built"
+    out = {}
+    xyz, val = cases.synth_data(11, 300, 2)
+    pts = cases.synth_points(11, 200, 2, xyz)
+    out["oracle/fp"] = np.array([xyz.sum(), val.sum(), pts.sum()])
+    for model in ("linear", "power", "gaussian", "exponential", "spherical"):
+        stored = ko.stored_parameters(model, cases.MODELS[model])
+        for exact in (True, False):
+            z, ss = rn.exec_loop(xyz, pts, val, model, stored, exact_values=exact)
+            out["oracle/%s/%d/z" % (model, exact)], out["oracle/%s/%d/ss" % (model, exact)] = z, ss
+    for dim, k in ((2, 8), (3, 12)):
+        xyz, val = cases.synth_data(12 + dim, 400, dim)
+        pts = cases.synth_points(12 + dim, 150, dim, xyz)
+        out["oracle_mw/%d/fp" % dim] = np.array([xyz.sum(), val.sum(), pts.sum()])
+        z, ss = rn.exec_loop_moving_window(xyz, pts, val, "exponential", ko.stored_parameters("exponential", [1.0, 150.0, 0.05]), k)
+        out["oracle_mw/%d/z" % dim], out["oracle_mw/%d/ss" % dim] = z, ss
+    xyz, val = cases.synth_data(2024, 1500, 2)
+    pts = cases.synth_points(2024, 2000, 2, xyz)
+    out["cuda/fp"] = np.array([xyz.sum(), val.sum(), pts.sum()])
+    for model in ("exponential", "spherical", "linear"):
+        z, ss = rn.exec_loop(xyz, pts, val, model, ko.stored_parameters(model, cases.MODELS[model]))
+        out["cuda/%s/z" % model], out["cuda/%s/ss" % model] = z, ss
+    z, ss = rn.exec_loop_moving_window(xyz, pts, val, "exponential", ko.stored_parameters("exponential", [1.0, 150.0, 0.05]), 16)
+    out["cuda/knn/z"], out["cuda/knn/ss"] = z, ss
+    return out
+
+
 if __name__ == "__main__":
-    which = sys.argv[1:] or ["goldens", "cases", "ctor", "pinv", "scenarios", "custom", "vgfit", "api", "fuzz"]
+    which = sys.argv[1:] or ["goldens", "cases", "ctor", "pinv", "scenarios", "custom", "vgfit", "api", "fuzz", "twins"]
+    if "twins" in which:
+        ref_twins()
     if "fuzz" in which:
         ref_fuzz()
     if "api" in which:

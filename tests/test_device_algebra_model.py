@@ -217,7 +217,7 @@ def i8_matvec_rows(W, c, S):
         acc = np.zeros(W.shape[0], dtype=np.int64)
         for s in range(d + 1):
             acc += ws[s] @ cs[d - s]
-        assert np.abs(acc).max() < 2 ** 31, "int32 TMEM accumulator would overflow"
+        assert np.abs(acc).max() < 2 ** 31, "int32 accumulator would overflow"
         V = V * 128 + acc                                                                  # exact in int64
     return np.ldexp(V.astype(np.float64), ew + ec - 12 - 7 * (S - 1))
 
@@ -243,8 +243,8 @@ def test_int8_slice_scheme_is_error_free_and_fp64_class(S, bits, bound):
         exact = W @ c
         got = i8_matvec_rows(W, c, S)
         worst = max(worst, abs(np.sum(got ** 2) - np.sum(exact ** 2)) / np.sum(exact ** 2))
-    # relative error of q here: 1.8e-11 / 1.9e-9 / 1.9e-7; sigma^2 = c0 - q + ... loses another ~20x to cancellation (measured on the B200 at N=5000:
-    # 4e-10 / 1.3e-7 / 4e-6 on sigma^2 for S = 6 / 5 / 4)
+    # relative error of q here: 1.8e-11 / 1.9e-9 / 1.9e-7; sigma^2 = c0 - q + ... loses another ~20x to cancellation (bench.py on an
+    # H100 at N=5000: 4e-10 / 4e-6 on sigma^2 for S = 6 / 4)
     assert worst < bound, worst
 
 

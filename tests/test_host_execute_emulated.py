@@ -222,7 +222,7 @@ def test_verbose_constructors_with_a_device_present(monkeypatch, capsys):
     """verbose=True makes the UK / 3-D constructors compute the cross-validation statistics where the reference does
     (uk.py:380-394: BEFORE the drift terms are initialised). With a device present that goes through _ensure_problem,
     which must then describe the ordinary-kriging system — not trip over drift attributes that do not exist yet
-    (seen on the B200 box: AttributeError 'point_log_drift')."""
+    (seen with a device present: AttributeError 'point_log_drift')."""
     import pykrige_b200 as pk
     from pykrige_b200 import _cabi
     monkeypatch.setattr(_cabi, "Handle", EmulatedHandle)

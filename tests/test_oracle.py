@@ -1,11 +1,13 @@
 """CPU tests: the oracle (oracle/krige_oracle.py) is pinned against (a) the reference's own golden
 vectors and (b) outputs of the imported reference for every seeded case (tests/golden/*.npz)."""
+import os
+
 import numpy as np
 import pytest
 from numpy.testing import assert_allclose
 
 import cases
-from conftest import assert_parity
+from conftest import GOLDEN, assert_parity
 from oracle import krige_oracle as ko
 
 
@@ -181,36 +183,34 @@ def test_oracle_pseudo_inverse_known_answer(ptype):
     assert np.isclose(z[0], 2.0)
 
 
-# ---- the reference's compiled native twins (oracle/_ref, built by oracle/build_ref.py) ----------------
-def _native():
-    from oracle import ref_native
-    if not ref_native.available():
-        pytest.skip("oracle/_ref is not built (python oracle/build_ref.py, needs /root/reference)")
-    return ref_native
+# ---- the reference's compiled native twins (their outputs stored by tests/golden/make_golden.py twins) ----------
+@pytest.fixture(scope="module")
+def ref_twins():
+    return np.load(os.path.join(GOLDEN, "ref_twins.npz"))
 
 
 @pytest.mark.parametrize("model", ["linear", "power", "gaussian", "exponential", "spherical"])
-def test_oracle_matches_compiled_reference_twin(model):
+def test_oracle_matches_compiled_reference_twin(model, ref_twins):
     """The numpy restatement vs the reference's own compiled `_c_exec_loop` (cok.pyx:14-96), same inputs."""
-    rn = _native()
     xyz, val = cases.synth_data(11, 300, 2)
     pts = cases.synth_points(11, 200, 2, xyz)
+    assert_allclose([xyz.sum(), val.sum(), pts.sum()], ref_twins["oracle/fp"], rtol=1e-12)
     stored = ko.stored_parameters(model, cases.MODELS[model])
     for exact in (True, False):
-        z, ss = rn.exec_loop(xyz, pts, val, model, stored, exact_values=exact)
+        z, ss = ref_twins["oracle/%s/%d/z" % (model, exact)], ref_twins["oracle/%s/%d/ss" % (model, exact)]
         zo, so = ko.krige(xyz, val, model, stored, pts, exact_values=exact)
         assert_parity(zo, z, 1e-8, "z")
         assert_parity(so, ss, 1e-8, "ss")
 
 
-def test_oracle_moving_window_matches_compiled_reference_twin():
+def test_oracle_moving_window_matches_compiled_reference_twin(ref_twins):
     """... and `_c_exec_loop_moving_window` (cok.pyx:98-193), 2-D and 3-D."""
-    rn = _native()
     for dim, k in ((2, 8), (3, 12)):
         xyz, val = cases.synth_data(12 + dim, 400, dim)
         pts = cases.synth_points(12 + dim, 150, dim, xyz)
+        assert_allclose([xyz.sum(), val.sum(), pts.sum()], ref_twins["oracle_mw/%d/fp" % dim], rtol=1e-12)
         stored = ko.stored_parameters("exponential", [1.0, 150.0, 0.05])
-        z, ss = rn.exec_loop_moving_window(xyz, pts, val, "exponential", stored, k)
+        z, ss = ref_twins["oracle_mw/%d/z" % dim], ref_twins["oracle_mw/%d/ss" % dim]
         zo, so = ko.krige(xyz, val, "exponential", stored, pts, n_closest_points=k)
         assert_parity(zo, z, 1e-9, "z")
         assert_parity(so, ss, 1e-9, "ss")

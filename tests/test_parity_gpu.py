@@ -1,15 +1,17 @@
-"""GPU parity tests (run with -m gpu on a B200): backend='cuda' through the C ABI vs
+"""GPU parity tests (run with -m gpu on an H100): backend='cuda' through the C ABI vs
  (a) the committed outputs of the imported reference (tests/golden/ref_cases.npz),
  (b) the reference's own golden vectors (tests/golden/reference_goldens.npz),
  (c) the CPU oracle on fresh seeded inputs, and size-independent properties at larger sizes.
 Tolerance (BASELINE.json north_star / SURVEY.md §8d): rtol = 1e-5, atol = 1e-5*max|ref| for fp64.
 """
+import os
+
 import numpy as np
 import pytest
 from numpy.testing import assert_allclose
 
 import cases
-from conftest import assert_parity
+from conftest import GOLDEN, assert_parity
 
 pytestmark = pytest.mark.gpu
 R64 = 1e-5
@@ -402,7 +404,7 @@ def test_intermediates_match_scipy(pk):
     assert_allclose(np.tril(W), sl.solve_triangular(Lr, np.eye(n), lower=True), rtol=1e-7, atol=1e-10)
 
 
-# ---- fp32 device math (tcgen05 kind::tf32, 3xTF32 split): tolerance rtol = 1e-2 (north_star) ----------
+# ---- fp32 device math (wgmma .tf32, 3xTF32 split): tolerance rtol = 1e-2 (north_star) ----------
 R32 = 1e-2
 F32_CASES = [c for c in GLOBAL_CASES if c["name"] in (
     "cfg1_ok2d_n100_grid50", "ok2d_exponential_aniso", "ok2d_gaussian_aniso", "ok2d_spherical_aniso",
@@ -737,27 +739,25 @@ def test_whole_chain_scenarios_match_reference(pk, sc, ref_scenarios, ref_golden
                         atol=1e-5 * np.abs(ref_scenarios[sc["name"] + "/epsilon"]).max())
 
 
-# ---- straight against the reference's compiled native code (oracle/_ref travels to the GPU box) ---------
+# ---- straight against the outputs of the reference's compiled native code (tests/golden/ref_twins.npz) ---------
 def test_cuda_matches_compiled_reference_twins(pk):
-    """backend='cuda' vs the reference's own `_c_exec_loop` / `_c_exec_loop_moving_window` (lib/cok.pyx,
-    compiled by oracle/build_ref.py) on fresh seeded inputs — no committed fixture in between."""
-    from oracle import ref_native as rn, krige_oracle as ko
-    if not rn.available():
-        pytest.skip("oracle/_ref is not built")
+    """backend='cuda' vs the reference's own `_c_exec_loop` / `_c_exec_loop_moving_window` (lib/cok.pyx, compiled by
+    oracle/build_ref.py; outputs stored by tests/golden/make_golden.py twins) on seeded inputs."""
+    ref = np.load(os.path.join(GOLDEN, "ref_twins.npz"))
     xyz, val = cases.synth_data(2024, 1500, 2)
     pts = cases.synth_points(2024, 2000, 2, xyz)
+    assert_allclose([xyz.sum(), val.sum(), pts.sum()], ref["cuda/fp"], rtol=1e-12)
     for model in ("exponential", "spherical", "linear"):
         params = cases.MODELS[model]
         m = pk.OrdinaryKriging(xyz[:, 0], xyz[:, 1], val, variogram_model=model, variogram_parameters=list(params))
         z, ss = m.execute("points", pts[:, 0], pts[:, 1], backend="cuda")
-        zr, sr = rn.exec_loop(xyz, pts, val, model, ko.stored_parameters(model, params))
+        zr, sr = ref["cuda/%s/z" % model], ref["cuda/%s/ss" % model]
         assert_parity(z, zr, R64, model + " z vs cok._c_exec_loop")
         assert_parity(ss, sr, R64, model + " ss vs cok._c_exec_loop")
     m = pk.OrdinaryKriging(xyz[:, 0], xyz[:, 1], val, variogram_model="exponential",
                            variogram_parameters=[1.0, 150.0, 0.05])
     z, ss = m.execute("points", pts[:, 0], pts[:, 1], backend="cuda", n_closest_points=16)
-    zr, sr = rn.exec_loop_moving_window(xyz, pts, val, "exponential",
-                                        ko.stored_parameters("exponential", [1.0, 150.0, 0.05]), 16)
+    zr, sr = ref["cuda/knn/z"], ref["cuda/knn/ss"]
     assert_parity(z, zr, R64, "knn z vs cok._c_exec_loop_moving_window")
     assert_parity(ss, sr, R64, "knn ss vs cok._c_exec_loop_moving_window")
 
@@ -868,7 +868,7 @@ def test_custom_variogram_cases_match_reference(pk, case, ref_custom):
 
 
 def test_custom_variogram_other_dtypes(pk, ref_custom):
-    """The tabulated model also feeds the tcgen05 kernels (float32 3xTF32, float64x INT8 slices)."""
+    """The tabulated model also feeds the wgmma kernels (float32 3xTF32, float64x INT8 slices)."""
     case = cases.CUSTOM_CASES[0]
     inp = cases.build_inputs(case)
     m = cases.make_model(pk, case, inp)

@@ -1,4 +1,4 @@
-"""GPU parity on randomised configurations (run with -m gpu on a B200): the 240 whole-execute() draws of
+"""GPU parity on randomised configurations (run with -m gpu on an H100): the 240 whole-execute() draws of
 tests/cases.py fuzz_config — the four classes x grid / masked / points x every drift kind x anisotropy x exact_values x
 moving window, masks and specified-drift arrays also in the transposed orientation the reference tolerates, rasters with
 a descending axis, exact hits, 1 x 1 grids, as few as 8 data points — through the C ABI against the outputs of the
