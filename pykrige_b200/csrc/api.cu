@@ -14,8 +14,8 @@
 
 #define KB_VERSION 2000
 static const int64_t KB_STAGE_PTS = 1 << 20;   // prediction points per staged output chunk (2 x 8 MB through pinned memory)
-#define KB_TILE_COST_32 0.540     // one round of 32-point tiles relative to one round of 64-point tiles (fp64 kernel, N=5000,
-#define KB_TILE_COST_16 0.309     // one H100 at 400 W: 8.11 / 4.38 / 2.51 ms per round; scripts/tile_timing.py)
+#define KB_TILE_COST_32 0.607     // one round of 32-point tiles relative to one round of 64-point tiles (fp64 kernel, N=5000,
+#define KB_TILE_COST_16 0.403     // one H100 80GB HBM3 at 400 W: 5.26 / 3.19 / 2.12 ms per round; scripts/tile_timing.py)
 static const int64_t KB_STAGE_MIN = 1 << 18;   // below this the outputs go straight to the caller's buffers
 
 struct Src {

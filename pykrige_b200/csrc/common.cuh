@@ -213,6 +213,22 @@ __device__ __forceinline__ void kb_dmma(double& c0, double& c1, double a, double
                  : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
 }
 
+// ---- mma.sync m16n8k4 f64 (SASS DMMA.16x8x4): the shape of the fp64 solve kernel --------------------------------
+// g = lane >> 2, t = lane & 3.  A 16x4 row: a[i] = A[g + 8 i][t];  B 4x8 col: b = B[t][g];  C 16x8: c[i] = C[g + 8 (i >> 1)][2t + (i & 1)]
+// (tests/test_dmma_fragments_gpu.py pins these maps). On H100 the 16x8xK shapes run at twice the per-FMA rate of
+// m8n8k4 (scripts/dmma_rate.py); k = 4 keeps the operand registers per MMA smallest.
+__device__ __forceinline__ void kb_dmma_16x8x4(double* c, const double* a, double b) {
+    asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+                 : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+                 : "d"(a[0]), "d"(a[1]), "d"(b));
+}
+
+// W tile order of the fp64 solve kernel (KB_BM x KB_BK, element (r, k)):  [m16 tile r/16][k/4][lane (r%8)*4 + k%4][(r/8)%2]
+// = the m16n8k4 A fragment (rows g and g + 8) of each lane as one double2, so one LDS.128 over the 32 lanes reads 512
+// contiguous bytes (conflict-free); written by pack_kernel<double> / pack_gform_kernel (factor.cu). The RHS tile keeps
+// the m8n8k4-era order ((k/4)*NT + n/8)*32 + (n%8)*4 + k%4, which already is the m16n8k4 B fragment: one LDS.64 over
+// 256 contiguous bytes.
+
 // ---- L2 cache policies for the bulk copies of the solve kernels ----------------------------------------------
 // The factor tile stream (W) is read by every CTA for every point tile: keep what L2 holds of it (evict_last; DESIGN.md §2
 // has the measurement on H100, where W outgrows L2 above N ~ 3500). The per-CTA

@@ -589,8 +589,20 @@ __global__ void __launch_bounds__(256) dual_small_kernel(int n, int n_pad, int K
 
 // ---------------------------------------------------------------------------
 // K2d  pack: tile (row block I, k tile kt) -> 4096 values in fragment order
-//   element (r, k) of the tile lives at ((k/4)*32 + r/8)*32 + (r%8)*4 + k%4
+//   double (the fp64 DMMA solve kernel): element (r, k) of the tile lives at ((r/16)*4 + k/4)*64 + ((r%8)*4 + k%4)*2 +
+//   (r/8)%2, the m16n8k4 A-fragment order of common.cuh; float: ((k/4)*32 + r/8)*32 + (r%8)*4 + k%4
 // rows < n: W (lower triangle); rows [n, n+na): dual rows Uz^T; other rows 0.
+__device__ __forceinline__ void pack_rk(bool f64, int I, int kt, int e, int& r, int& k) {
+    if (f64) {       // e = ((m16 tile * 4 + k/4) * 32 + lane) * 2 + (r/8)%2, lane = (r%8)*4 + k%4
+        const int h = e & 1, lane = (e >> 1) & 31, k4 = (e >> 6) & 3, mt = e >> 8;
+        r = I * KB_BM + mt * 16 + 8 * h + (lane >> 2);
+        k = kt * KB_BK + k4 * 4 + (lane & 3);
+    } else {
+        const int lane = e & 31, mt = (e >> 5) & 31, k4 = e >> 10;
+        r = I * KB_BM + mt * 8 + (lane >> 2);
+        k = kt * KB_BK + k4 * 4 + (lane & 3);
+    }
+}
 template <typename T>
 __global__ void __launch_bounds__(256) pack_kernel(const double* __restrict__ W, int ld, int n, int n_pad, int na,
                                                     const double* __restrict__ Uz, PackMap pm, T* __restrict__ out) {
@@ -598,9 +610,8 @@ __global__ void __launch_bounds__(256) pack_kernel(const double* __restrict__ W,
     if (kt >= pm.ktiles[I]) return;
     T* o = out + ((size_t)pm.tile_off[I] + kt) * (KB_BM * KB_BK);
     for (int e = threadIdx.x; e < KB_BM * KB_BK; e += 256) {
-        int lane = e & 31, mt = (e >> 5) & 31, k4 = e >> 10;
-        int r = I * KB_BM + mt * 8 + (lane >> 2);
-        int k = kt * KB_BK + k4 * 4 + (lane & 3);
+        int r, k;
+        pack_rk(sizeof(T) == sizeof(double), I, kt, e, r, k);
         double v = 0.0;
         if (r < n) { if (k <= r) v = W[(size_t)r * ld + k]; }
         else if (r < n + na) { if (k < n) v = Uz[(size_t)(r - n) * n_pad + k]; }
@@ -857,9 +868,8 @@ __global__ void __launch_bounds__(256) pack_gform_kernel(const double* __restric
     if (kt >= pm.ktiles[I]) return;
     double* o = out + ((size_t)pm.tile_off[I] + kt) * (KB_BM * KB_BK);
     for (int e = threadIdx.x; e < KB_BM * KB_BK; e += 256) {
-        int lane = e & 31, mt = (e >> 5) & 31, k4 = e >> 10;
-        int r = I * KB_BM + mt * 8 + (lane >> 2);
-        int k = kt * KB_BK + k4 * 4 + (lane & 3);
+        int r, k;
+        pack_rk(true, I, kt, e, r, k);           // fp64 solve kernel order, as pack_kernel<double>
         double v = 0.0;
         if (r < n) {
             if (k < r) v = G[(size_t)r * ld + k] + G[(size_t)k * ld + r];

@@ -8,7 +8,8 @@
 //     g_j  = U^T c_j, zc_j = zeta . c_j   <- extra dense "dual rows" appended to W (same GEMM)
 //     finalize: r = g - f_j, mu = S^-1 r, sigma2 = c0 - q + r.mu, z = zc - mu.phi
 //
-// Kernels in this file (all fp64, mma.sync.m8n8k4 = SASS DMMA):
+// Kernels in this file (all fp64, mma.sync.m16n8k4 = SASS DMMA.16x8x4; on H100 the 16x8xK shapes run at twice the
+// per-FMA rate of m8n8k4, 127 vs 64 FMA/clk/SM, scripts/dmma_rate.py):
 //   solve_kernel_pt   (K3 v3, the product path) persistent CTAs, one CTA = 64 points x all rows of W, RHS column
 //                     block generated once per tile, W/RHS tiles streamed by cp.async.bulk + mbarrier, fused
 //                     finalize. See the comment above the kernel.
@@ -57,16 +58,55 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
 //            park it, already in MMA-fragment order, in a per-CTA scratch ring (L2-resident, re-used for
 //            every tile the CTA processes; size independent of M);
 //   phase M  warp 0 streams W tiles (32 KB) and RHS tiles (8 KB) with cp.async.bulk + mbarrier into a
-//            4-stage ring; warps 4..11 do nothing but LDS + DMMA, walking all row blocks and keeping the
-//            per-point sum of squares in registers;
+//            5-stage ring; warps 4..11 do nothing but LDS + m16n8k4 DMMA, walking all row blocks; each owns
+//            the 16-row m-tiles j and 15 - j of a block (2 x NT x 4 accumulators) and adds its per-point sums
+//            of squares to shared memory at the end of every row block (registers go to the accumulators:
+//            a CTA of 12 warps gets 168 per thread, and fewer warps would not raise that, as three warps
+//            still share one SM sub-partition's 64 KB register file);
 //   phase F  the (K+1)x(K+1) drift solve and the two outputs per point are produced in the same CTA:
 //            no partial buffers, no separate finalize pass, fixed summation order (deterministic).
 #define PT_STAGES 5
 #define PT_THREADS 384
+#define PT_CONS0 (PT_THREADS / 32 - 8)    // first of the 8 consumer warps
 #define PT_STAGE_BYTES ((KB_BM * KB_BK + KB_BK * KB_TN) * 8)
 
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" :: "r"(smem_u32(bar)) : "memory");
+}
+
+// Sum of v[0..CNT) over the 8 lanes of a warp that share lane & 3 (the row lanes of an MMA C fragment), halving the
+// values at each of the butterfly steps xor 16, 8, 4: afterwards v[0..max(CNT/8, 1)) hold this lane's share of the sums.
+// Every sum is added up in the same tree ((l + l^16) + (l^8 + ...)) + ... whatever CNT is, so a point's result does
+// not depend on the tile width.
+template <int C>
+__device__ __forceinline__ void pt_reduce_scatter_step(double* v, int lane, int mask) {
+    if constexpr (C >= 2) {
+        const bool up = (lane & mask) != 0;
+#pragma unroll
+        for (int h = 0; h < C / 2; ++h) {
+            const double send = up ? v[h] : v[h + C / 2];
+            const double keep = up ? v[h + C / 2] : v[h];
+            v[h] = keep + __shfl_xor_sync(0xffffffffu, send, mask);
+        }
+    } else {
+        v[0] += __shfl_xor_sync(0xffffffffu, v[0], mask);
+    }
+}
+template <int CNT>
+__device__ __forceinline__ void pt_reduce_scatter(double* v, int lane) {
+    pt_reduce_scatter_step<CNT>(v, lane, 16);
+    pt_reduce_scatter_step<(CNT >= 2 ? CNT / 2 : 1)>(v, lane, 8);
+    pt_reduce_scatter_step<(CNT >= 4 ? CNT / 4 : 1)>(v, lane, 4);
+}
+// which of the CNT sums v[i] holds after pt_reduce_scatter<CNT> (-1: a duplicate another lane also holds)
+template <int CNT>
+__device__ __forceinline__ int pt_reduce_scatter_index(int i, int lane) {
+    int o = i, c = CNT;
+    for (int mask = 16; mask >= 4; mask >>= 1) {
+        if (c >= 2) { c /= 2; if (lane & mask) o += c; }
+        else if (lane & mask) return -1;
+    }
+    return o;
 }
 
 // NT = n-tiles (of 8 points) per point tile: 8 (64 points) is the default. Narrower tiles (NT = 4, 2: 32 / 16 points) are used by
@@ -98,10 +138,16 @@ __global__ void __launch_bounds__(PT_THREADS, 1) solve_kernel_pt(const __grid_co
     }
     __syncthreads();
 
-    uint32_t git = 0;                 // running stage counter (same sequence in producer and consumers)
-    const int cw = warp - 4;          // consumer warp 0..7
+    // stages of one tile (W tiles of all row blocks); the running stage counter of a tile starts at (tiles this CTA
+    // already did) x this, the same sequence in producer and consumers (recomputed per tile: no register held)
+    const uint32_t stages_per_tile = (uint32_t)(P.pm.tile_off[P.nrb - 1] + P.pm.ktiles[P.nrb - 1]);
+    const int cw = warp - PT_CONS0;   // consumer warp 0..7
 
-    for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    // the loop counts this CTA's tiles in 32 bits and forms the 64-bit tile index where it is used: registers are
+    // scarce in phase M (the accumulators take 128 of the 168)
+    for (uint32_t it = 0; blockIdx.x + (long long)it * gridDim.x < ntiles; ++it) {
+        const long long tile = blockIdx.x + (long long)it * gridDim.x;
+        const uint32_t git = it * stages_per_tile;
         // ---------------- phase G: RHS column block of this tile, once ----------------
         {
             const int pl = tid % TN;                 // point within the tile
@@ -157,110 +203,123 @@ __global__ void __launch_bounds__(PT_THREADS, 1) solve_kernel_pt(const __grid_co
                     }
                 }
             }
-        } else if (warp >= 4) {
+        } else if (warp >= PT_CONS0) {
             uint32_t g = git;
-            double qs[NT][2];
+            // running per-point sums of this warp, kept in its row of qred (registers are spent on the accumulators):
+            // after the reduce-scatter of each row-block epilogue, sum v of this lane belongs to (n-tile, column)
+            // o = pt_reduce_scatter_index(v), or is a duplicate another lane owns (o < 0)
+            constexpr int QV = NT >= 4 ? NT / 4 : 1;
+            double* qrow = qred + cw * TN;
 #pragma unroll
-            for (int nt = 0; nt < NT; ++nt) { qs[nt][0] = 0.0; qs[nt][1] = 0.0; }
+            for (int v = 0; v < QV; ++v) {
+                const int o = pt_reduce_scatter_index<2 * NT>(v, lane);     // sum 2 nt + i: point nt*8 + 2 t + i
+                if (o >= 0) qrow[(o >> 1) * 8 + 2 * (lane & 3) + (o & 1)] = 0.0;
+            }
+            // this warp owns the 16-row m-tiles cw and 15 - cw of every 256-row block: the pair keeps the eight warps
+            // equally busy inside the triangular diagonal block (cw + 1 and 16 - cw k tiles), and every m-tile skips
+            // the k tiles above its diagonal (W rows are lower-triangular, the dual rows dense, padding rows empty)
+            const int mtl[2] = {cw, 15 - cw};
             for (int I = 0; I < P.nrb; ++I) {
-                const int kt = P.pm.ktiles[I];
-                // this warp owns the m-tiles cw, cw+8, cw+16, cw+24 of the 256-row block (8 rows each):
-                // interleaving keeps the eight warps equally busy inside the triangular diagonal block and
-                // lets every m-tile skip the k tiles above the diagonal (W rows are lower-triangular, the
-                // dual rows are dense, padding rows need nothing)
-                int kmax[4];
+                const uint32_t gend = g + (uint32_t)P.pm.ktiles[I];
+                // stage counter bound of each m-tile: its k tiles 0 .. (k up to its last row) of the block
+                uint32_t glim[2];
 #pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const int r0 = I * KB_BM + (cw + 8 * q) * 8;
-                    if (r0 + 7 >= P.n && r0 < P.n + P.na) kmax[q] = 0x7fffffff;
-                    else if (r0 >= P.n + P.na) kmax[q] = -1;
-                    else kmax[q] = r0 + 7;
+                for (int q = 0; q < 2; ++q) {
+                    const int r0 = I * KB_BM + mtl[q] * 16;
+                    if (r0 + 15 >= P.n && r0 < P.n + P.na) glim[q] = gend;
+                    else if (r0 >= P.n + P.na) glim[q] = g;
+                    else glim[q] = g + (uint32_t)(r0 / KB_BK + 1);
                 }
-                double acc[4][NT][2];
+                double acc[2][NT][4];
 #pragma unroll
-                for (int a = 0; a < 4; ++a)
+                for (int a = 0; a < 2; ++a)
 #pragma unroll
-                    for (int b = 0; b < NT; ++b) { acc[a][b][0] = 0.0; acc[a][b][1] = 0.0; }
-                for (int t = 0; t < kt; ++t, ++g) {
+                    for (int b = 0; b < NT; ++b)
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) acc[a][b][i] = 0.0;
+                for (; g < gend; ++g) {
                     const int s = g % PT_STAGES;
                     // every consumer waits for every stage (also the ones it skips) so that no warp can lap
                     // the ring and arrive twice on empty[s] within one phase
                     mbar_wait(&full[s], (uint32_t)((g / PT_STAGES) & 1));
-                    const int k0 = t * KB_BK;
-                    if (k0 <= kmax[3] || k0 <= kmax[2] || k0 <= kmax[1] || k0 <= kmax[0]) {
-                        const double* ts = Ts + (size_t)s * KB_BM * KB_BK;
+                    const bool on0 = g < glim[0], on1 = g < glim[1];
+                    if (on0 || on1) {
+                        const double2* ts = reinterpret_cast<const double2*>(Ts + (size_t)s * KB_BM * KB_BK);
                         const double* bs = Bs + (size_t)s * KB_BK * TN;
 #pragma unroll
-                        for (int k4 = 0; k4 < 4; ++k4) {
-                            double fb[NT];
+                        for (int k4 = 0; k4 < 4; ++k4) {         // four m16n8k4 steps per k tile, k ascending
+                            double fa[2][2];
 #pragma unroll
-                            for (int nt = 0; nt < NT; ++nt) fb[nt] = bs[(k4 * NT + nt) * 32 + lane];
+                            for (int q = 0; q < 2; ++q) {
+                                const double2 v = ts[(mtl[q] * 4 + k4) * 32 + lane];
+                                fa[q][0] = v.x; fa[q][1] = v.y;
+                            }
 #pragma unroll
-                            for (int q = 0; q < 4; ++q) {
-                                if (k0 <= kmax[q]) {
-                                    const double fa = ts[(k4 * 32 + cw + 8 * q) * 32 + lane];
-#pragma unroll
-                                    for (int nt = 0; nt < NT; ++nt)
-                                        kb_dmma(acc[q][nt][0], acc[q][nt][1], fa, fb[nt]);
-                                }
+                            for (int nt = 0; nt < NT; ++nt) {
+                                const double fb = bs[(k4 * NT + nt) * 32 + lane];
+                                if (on0) kb_dmma_16x8x4(acc[0][nt], fa[0], fb);
+                                if (on1) kb_dmma_16x8x4(acc[1][nt], fa[1], fb);
                             }
                         }
                     }
                     __syncwarp();
                     if (lane == 0) mbar_arrive(&empty[s]);
                 }
-                // row-block epilogue: W rows -> running sum of squares; dual rows -> shared memory
+                // row-block epilogue, in place: every accumulator of a W row becomes its term of the point's sum (square,
+                // or c[r] times it for the quadratic form), dual rows go to shared memory and, like padding rows, add 0;
+                // then the warp's per-point sums (fixed order: m-tile, row g before g + 8) are reduced over the 8 row
+                // lanes and added to the running sums
 #pragma unroll
-                for (int mt = 0; mt < 4; ++mt) {
-                    const int r = I * KB_BM + (cw + 8 * mt) * 8 + (lane >> 2);
-                    if (r < P.n) {
-                        if (!P.gform) {
+                for (int q = 0; q < 2; ++q)
 #pragma unroll
-                            for (int nt = 0; nt < NT; ++nt) {
-                                qs[nt][0] += acc[mt][nt][0] * acc[mt][nt][0];
-                                qs[nt][1] += acc[mt][nt][1] * acc[mt][nt][1];
+                    for (int h = 0; h < 2; ++h) {
+                        const int r = I * KB_BM + mtl[q] * 16 + 8 * h + (lane >> 2);
+                        if (r < P.n) {
+                            if (!P.gform) {
+#pragma unroll
+                                for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+                                    for (int i = 0; i < 2; ++i) acc[q][nt][2 * h + i] *= acc[q][nt][2 * h + i];
+                            } else {
+                                // quadratic form c^T G c: multiply row r of T c by c[r] (read back from the scratch
+                                // ring: tile r/16, fragment order)
+                                const double* bt = P.scratch + ((size_t)blockIdx.x * nk + (r >> 4)) * (KB_BK * TN) +
+                                                   ((r & 15) >> 2) * (NT * 32) + (r & 3);
+#pragma unroll
+                                for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+                                    for (int i = 0; i < 2; ++i) {
+                                        const int c = nt * 8 + 2 * (lane & 3) + i;
+                                        acc[q][nt][2 * h + i] *= bt[(c >> 3) * 32 + (c & 7) * 4];
+                                    }
                             }
                         } else {
-                            // quadratic form c^T G c: multiply row r of T c by c[r] (read back from the
-                            // scratch ring: tile r/16, fragment order)
-                            const double* bt = scratch + (size_t)(r >> 4) * (KB_BK * TN) + ((r & 15) >> 2) * (NT * 32) + (r & 3);
+                            if (r < P.n + P.na) {
+                                double* ao = auxs + (r - P.n) * TN + 2 * (lane & 3);
 #pragma unroll
-                            for (int nt = 0; nt < NT; ++nt) {
-                                const int c0i = nt * 8 + 2 * (lane & 3);
-                                qs[nt][0] += acc[mt][nt][0] * bt[(c0i >> 3) * 32 + (c0i & 7) * 4];
-                                qs[nt][1] += acc[mt][nt][1] * bt[((c0i + 1) >> 3) * 32 + ((c0i + 1) & 7) * 4];
+                                for (int nt = 0; nt < NT; ++nt) {
+                                    ao[nt * 8] = acc[q][nt][2 * h];
+                                    ao[nt * 8 + 1] = acc[q][nt][2 * h + 1];
+                                }
                             }
-                        }
-                    } else if (r < P.n + P.na) {
-                        double* ao = auxs + (r - P.n) * TN + 2 * (lane & 3);
 #pragma unroll
-                        for (int nt = 0; nt < NT; ++nt) {
-                            ao[nt * 8] = acc[mt][nt][0];
-                            ao[nt * 8 + 1] = acc[mt][nt][1];
+                            for (int nt = 0; nt < NT; ++nt) { acc[q][nt][2 * h] = 0.0; acc[q][nt][2 * h + 1] = 0.0; }
                         }
                     }
-                }
-            }
+                double part[2 * NT];
 #pragma unroll
-            for (int nt = 0; nt < NT; ++nt)
+                for (int nt = 0; nt < NT; ++nt)
 #pragma unroll
-                for (int i = 0; i < 2; ++i) {
-                    double v = qs[nt][i];
-                    v += __shfl_xor_sync(0xffffffffu, v, 4);
-                    v += __shfl_xor_sync(0xffffffffu, v, 8);
-                    v += __shfl_xor_sync(0xffffffffu, v, 16);
-                    qs[nt][i] = v;
-                }
-            if ((lane >> 2) == 0) {
+                    for (int i = 0; i < 2; ++i)
+                        part[2 * nt + i] = ((acc[0][nt][i] + acc[0][nt][2 + i]) + acc[1][nt][i]) + acc[1][nt][2 + i];
+                pt_reduce_scatter<2 * NT>(part, lane);
 #pragma unroll
-                for (int nt = 0; nt < NT; ++nt) {
-                    qred[cw * TN + nt * 8 + 2 * lane] = qs[nt][0];
-                    qred[cw * TN + nt * 8 + 2 * lane + 1] = qs[nt][1];
+                for (int v = 0; v < QV; ++v) {
+                    const int o = pt_reduce_scatter_index<2 * NT>(v, lane);
+                    if (o >= 0) qrow[(o >> 1) * 8 + 2 * (lane & 3) + (o & 1)] += part[v];
                 }
             }
         }
-        // every role advances the ring counter by the same amount
-        for (int I = 0; I < P.nrb; ++I) git += (uint32_t)P.pm.ktiles[I];
         __syncthreads();
 
         // ---------------- phase F: per-point finalize (DESIGN.md §3) ----------------
