@@ -69,6 +69,9 @@ extern "C" {
 #define KB200_GEOGRAPHIC 1   /* (x, y) = (lon, lat) degrees; great-circle distances, core.py:36-97; OK 2-D only */
 
 #define KB200_MAX_DRIFT 15   /* drift columns (regional-linear + host supplied), excluding the unbiasedness column */
+#define KB200_MAX_FIELDS 64  /* value columns of one kb200_set_values problem: K + 1 + 64 <= 80 dual rows stay inside
+                                one extra 256-row block, and the moving window's augmented rows [c; 1; Z_1..Z_64] fit
+                                nine 8-row tiles (145 KB of shared memory per point at k = 128) */
 
 typedef struct kb200_ctx* kb200_handle;
 
@@ -309,6 +312,19 @@ int kb200_set_variogram_table(kb200_handle h, int64_t n_nodes, double dmax, cons
  */
 int kb200_set_pseudo_inverse(kb200_handle h, int enable);
 
+/* Several value fields on the same stations and variogram. The NEXT kb200_set_problem / kb200_set_problem_knn on this
+ * handle kriges the n_fields columns of `values` (host, column-major n x n_fields, copied) instead of its own `values`
+ * argument; the factorisation, the contraction q = ||W c||^2 and sigma^2 are shared, each field adds one dual row
+ * (zeta_v = C^-1 Z_v, DESIGN.md §5d). Every following execute call (host and _dev, points, grid and moving window)
+ * writes z_out as n_fields consecutive blocks of `count` values, field f at z_out + f * count, and ss_out once.
+ * Field f's results are bit-identical to a single-field problem with values = column f, whatever n_fields is.
+ * n_fields = 0 switches the feature off. Resets the handle's problem state.
+ * Errors: KB200_EBADARG for n_fields outside [0, KB200_MAX_FIELDS], n < 1, a NULL array or a non-finite value, and
+ * from kb200_set_problem* when n differs from the problem's n; KB200_EUNSUPPORTED from kb200_set_problem for a dtype
+ * other than KB200_F64 or with the pseudo-inverse, from kb200_describe_problem / kb200_group_set_problem* (no blob
+ * or group form) and from kb200_statistics. */
+int kb200_set_values(kb200_handle h, int n_fields, int64_t n, const double* values);
+
 /* ---- constructor-side helpers (SURVEY.md 8f next-2) ----------------------------------------------
  *
  * kb200_experimental_variogram replaces the pdist binning of core._initialize_variogram_model
@@ -337,7 +353,9 @@ int kb200_statistics(kb200_handle h, double* delta, double* sigma);
 /* Debug/verification taps (used by tests only): copy device intermediates to host.
  *  what = 1: Cholesky factor L of the shifted covariance matrix (n_pad x n_pad, row-major, lower triangle valid)
  *  what = 2: W = inv(L) (same layout)
- *  what = 3: dual block: Uz (n x (K+2), column-major), then Sinv ((K+1)^2), then phi (K+1), then c0
+ *  what = 3: dual block: Uz (n_pad x (K+1+V), column-major: C^-1 F for the K+1 drift and unbiasedness columns, then
+ *            zeta_v = C^-1 Z_v for the V value fields, V = 1 without kb200_set_values), then Sinv ((K+1)^2), then
+ *            phi_1 .. phi_V (K+1 each, phi_v = F^T zeta_v), then c0
  * `cap` is the capacity of `out` in doubles; returns the number of doubles written or a negative code. */
 int64_t kb200_debug_fetch(kb200_handle h, int what, double* out, int64_t cap);
 

@@ -303,7 +303,7 @@ class KrigeBase:
                 hsh.update(np.ascontiguousarray(a, dtype=np.float64).tobytes())
         return hsh.hexdigest()
 
-    def _problem_signature(self, dtype, knn):
+    def _problem_signature(self, dtype, knn, fields=None):
         x, y, z, v, center, Mt = self._data_arrays()
         mid, vp = self._device_model()
         n_rl, cols = self._drift_spec()
@@ -312,7 +312,16 @@ class KrigeBase:
                 np.ravel(np.asarray(self.variogram_model_parameters, dtype=float)))
         return (dtype, knn, mid, tuple(vp), bool(self.exact_values), tuple(np.ravel(Mt)), tuple(center),
                 n_rl, len(cols), x.size, getattr(self, "coordinates_type", "euclidean"),
-                bool(getattr(self, "pseudo_inv", False)), self._device_drift_signature(), self._content_digest())
+                bool(getattr(self, "pseudo_inv", False)), self._device_drift_signature(), self._content_digest(),
+                self._fields_signature(fields))
+
+    @staticmethod
+    def _fields_signature(fields):
+        """(V, digest) of the value fields a problem kriges instead of the constructor's values; (0, None) without."""
+        if fields is None:
+            return 0, None
+        import hashlib
+        return fields.shape[0], hashlib.blake2b(np.ascontiguousarray(fields).tobytes(), digest_size=16).hexdigest()
 
     def _device_drift_signature(self):
         return ()
@@ -321,7 +330,7 @@ class KrigeBase:
         """Hook for drift terms evaluated on the device (UniversalKriging: point_log, external_Z)."""
         h.set_device_drift(None, None)
 
-    def _ensure_problem(self, dtype="float64", knn=False, n_gpus=None):
+    def _ensure_problem(self, dtype="float64", knn=False, n_gpus=None, fields=None):
         name = dtype if isinstance(dtype, str) and dtype in _cabi.DTYPES else str(np.dtype(dtype))
         dt = _cabi.DTYPES.get(name)
         if dt is None:
@@ -330,7 +339,7 @@ class KrigeBase:
         grouped = isinstance(h, _cabi.Group)
         if self._device_model()[0] == self.TABLE_MODEL_ID:
             self._table_dmax()                  # fixes the tabulated range before it enters the signature
-        key = self._problem_signature(dt, knn)
+        key = self._problem_signature(dt, knn, fields)
         if (self._kb_gkey if grouped else self._kb_key) == key:
             return h
         x, y, z, v, center, Mt = self._data_arrays()
@@ -348,6 +357,8 @@ class KrigeBase:
         if mid == self.TABLE_MODEL_ID:
             dmax = self._table_dmax()
             h.set_variogram_table(self._variogram_table(dmax), dmax)
+        if fields is not None or getattr(h, "n_fields", 0):
+            h.set_values(fields)
         if knn:
             h.set_problem_knn(self._ndim, x, y, z, v, center, Mt, mid, vp, self.exact_values, self.eps)
         else:
@@ -438,14 +449,49 @@ class KrigeBase:
 
     @staticmethod
     def _shape_output(style, z, ss, sizes, flat_mask):
-        """Masked wrap + reshape of execute() (ok.py:1012-1020, ok3d.py:924-932)."""
+        """Masked wrap + reshape of execute() (ok.py:1012-1020, ok3d.py:924-932). z may carry a leading field
+        axis (execute(values=...)); the grid mask is broadcast over it."""
         if style == "masked":
-            z = np.ma.array(z, mask=flat_mask)
+            zmask = flat_mask if np.ndim(z) == 1 else np.broadcast_to(flat_mask, np.shape(z)).copy()
+            z = np.ma.array(z, mask=zmask)
             ss = np.ma.array(ss, mask=flat_mask)
         if style in ["masked", "grid"]:
-            z = z.reshape(sizes[::-1])
+            z = z.reshape(np.shape(z)[:-1] + tuple(sizes[::-1]))
             ss = ss.reshape(sizes[::-1])
         return z, ss
+
+    # ---- execute(values=...): several value fields through one factorisation ---------------------------------
+    @staticmethod
+    def _fields_kw(fields):
+        """Keyword for _run_cuda: without fields the call is the single-field call, unchanged."""
+        return {} if fields is None else {"fields": fields}
+
+    def _check_values(self, values, dtype, n_closest_points, n_gpus):
+        """Validates the values= keyword of execute() after the reference's own argument checks. Returns
+        (fields as a (V, N) float64 array, whether values was 1-D), or (None, False) for values=None."""
+        if values is None:
+            return None, False
+        v = np.asarray(values)
+        n = np.size(self._data_arrays()[3])
+        if v.ndim not in (1, 2):
+            raise ValueError("values must have shape (N,) or (N, V), got %d dimensions" % v.ndim)
+        if v.shape[0] != n:
+            raise ValueError("values has %d rows; it needs one row per data point (N = %d), shape (N, V)"
+                             % (v.shape[0], n))
+        one = v.ndim == 1
+        v = v.reshape(n, -1).astype(np.float64)
+        if v.shape[1] == 0:
+            raise ValueError("values has no fields (V = 0)")
+        if not np.all(np.isfinite(v)):
+            raise ValueError("values must be finite")
+        name = dtype if isinstance(dtype, str) else str(np.dtype(dtype))
+        if name != "float64":
+            raise NotImplementedError("execute(values=...) runs in dtype='float64' only")
+        if bool(getattr(self, "pseudo_inv", False)) and n_closest_points is None:
+            raise NotImplementedError("execute(values=...) is not supported with pseudo_inv=True")
+        if n_gpus is not None and int(n_gpus) > 1:
+            raise NotImplementedError("execute(values=...) runs on one GPU (n_gpus > 1 is not supported)")
+        return np.ascontiguousarray(v.T), one
 
     # ---- the device run: plan (what to compute) -> run (one contiguous block of it) -> scatter ----
     def _plan(self, style, axes, mask, drift_at=None):
@@ -494,27 +540,40 @@ class KrigeBase:
     def _scatter(plan, z, ss):
         if not plan["scatter"]:
             return z, ss
-        zf = np.zeros(plan["npt"])
+        zf = np.zeros(np.shape(z)[:-1] + (plan["npt"],))
         sf = np.zeros(plan["npt"])
-        zf[plan["idx"]] = z
+        zf[..., plan["idx"]] = z
         sf[plan["idx"]] = ss
         return zf, sf
 
-    def _run_cuda(self, style, axes, mask, n_closest_points=None, drift_at=None, dtype="float64", n_gpus=None):
+    def _run_cuda(self, style, axes, mask, n_closest_points=None, drift_at=None, dtype="float64", n_gpus=None,
+                  fields=None):
         """axes: list of 1-D coordinate arrays [x, y(, z)] (grid axes or point lists, original coords).
         mask: flattened bool mask (True = skip) or None.  drift_at: callable(pts list, idx) -> [n_hd, m]
         host-supplied drift values at the given points, or None.  n_gpus: None/1 = this handle's device;
         G > 1 = single-process multi-GPU (one host thread, kb200_group_*: device 0 factors, peer copies of the
         factor blob, contiguous blocks of the work list, results gathered in the reference's order).
-        Returns flat (z, ss) of length npt in the reference's flattened order."""
+        fields: (V, N) value fields kriged instead of the constructor's values, or None.
+        Returns flat (z, ss) of length npt in the reference's flattened order; z is (V, npt) with fields.
+        More than _cabi.MAX_FIELDS fields run as chunks of that many, each its own problem (factorisation) and
+        execute; every field's result is independent of the chunk it is in."""
         knn = n_closest_points is not None
         nd = self._ndim
         if self._device_model()[0] == self.TABLE_MODEL_ID and all(np.size(a) for a in axes[:nd]):
             self._table_dmax([float(np.min(a)) for a in axes[:nd]], [float(np.max(a)) for a in axes[:nd]])
-        h = self._ensure_problem(dtype, knn, n_gpus=n_gpus)
+        if fields is None:
+            h = self._ensure_problem(dtype, knn, n_gpus=n_gpus)
+            plan = self._plan(style, axes, mask, drift_at)
+            z, ss = self._run_block(h, plan, 0, plan["count"], n_closest_points, drift_at)
+            return self._scatter(plan, z, ss)
         plan = self._plan(style, axes, mask, drift_at)
-        z, ss = self._run_block(h, plan, 0, plan["count"], n_closest_points, drift_at)
-        return self._scatter(plan, z, ss)
+        zs = []
+        for c0 in range(0, fields.shape[0], _cabi.MAX_FIELDS):
+            chunk = fields[c0:c0 + _cabi.MAX_FIELDS]
+            h = self._ensure_problem(dtype, knn, n_gpus=n_gpus, fields=chunk)
+            z, ss = self._run_block(h, plan, 0, plan["count"], n_closest_points, drift_at)
+            zs.append(np.reshape(z, (chunk.shape[0], -1)))
+        return self._scatter(plan, np.concatenate(zs), ss)
 
     @staticmethod
     def _check_backend(backend, what):

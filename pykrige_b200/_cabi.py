@@ -27,6 +27,7 @@ KB200_F64X4 = 4  # 4 slices = 27 bits
 DTYPES = {"float64": KB200_F64, "float32": KB200_F32, "float64x": KB200_F64X, "float64x5": KB200_F64X5,
           "float64x4": KB200_F64X4}
 MAX_DRIFT = 15
+MAX_FIELDS = 64  # KB200_MAX_FIELDS: value fields of one kb200_set_values problem
 
 # every symbol include/krige_b200.h declares (checked by tests/test_cabi.py)
 EXPORTS = [
@@ -38,7 +39,7 @@ EXPORTS = [
     "kb200_blob_bytes", "kb200_blob_ptr", "kb200_describe_problem", "kb200_blob_commit",
     "kb200_set_coordinates", "kb200_set_stream", "kb200_last_timings", "kb200_reset_counters", "kb200_debug_fetch",
     "kb200_experimental_variogram", "kb200_statistics", "kb200_set_pseudo_inverse",
-    "kb200_set_variogram_table", "kb200_set_device_drift",
+    "kb200_set_variogram_table", "kb200_set_device_drift", "kb200_set_values",
     "kb200_group_create", "kb200_group_destroy", "kb200_group_last_error", "kb200_group_size", "kb200_group_member",
     "kb200_group_set_problem", "kb200_group_set_problem_knn", "kb200_group_execute_points",
     "kb200_group_execute_grid", "kb200_group_execute_knn_points", "kb200_group_execute_knn_grid",
@@ -103,6 +104,7 @@ def load_library():
     lib.kb200_set_pseudo_inverse.argtypes = [h, i32]
     lib.kb200_set_variogram_table.argtypes = [h, i64, ctypes.c_double, dp]
     lib.kb200_set_device_drift.argtypes = [h, i32, dp, i64, i64, dp, dp, dp]
+    lib.kb200_set_values.argtypes = [h, i32, i64, dp]
     lib.kb200_group_create.argtypes = [ctypes.POINTER(h), i32, ctypes.POINTER(i32)]
     lib.kb200_group_destroy.argtypes = [h]
     lib.kb200_group_destroy.restype = None
@@ -167,6 +169,7 @@ class Handle:
 
     _PREFIX = "kb200_"
     _owned = True
+    n_fields = 0        # value fields of the problem (kb200_set_values): z comes back as n_fields blocks
 
     @classmethod
     def _borrowed(cls, lib, raw):
@@ -268,7 +271,7 @@ class Handle:
     def execute_points(self, px, py, pz=None, drift_pts=None):
         px, py, pz = _f64(px), _f64(py), _f64(pz)
         m = px.size
-        z = np.empty(m, dtype=np.float64)
+        z = np.empty(max(1, self.n_fields) * m, dtype=np.float64)
         ss = np.empty(m, dtype=np.float64)
         dpts = _f64(drift_pts)
         self._check(self._fn("execute_points")(self._h, m, _ptr(px), _ptr(py), _ptr(pz), _ptr(dpts),
@@ -280,7 +283,7 @@ class Handle:
         nx, ny, nz = gx.size, gy.size, (gz.size if gz is not None else 1)
         if count is None:
             count = nx * ny * nz - first
-        z = np.empty(count, dtype=np.float64)
+        z = np.empty(max(1, self.n_fields) * count, dtype=np.float64)
         ss = np.empty(count, dtype=np.float64)
         dpts = _f64(drift_pts)
         self._check(self._fn("execute_grid")(self._h, nx, ny, nz, _ptr(gx), _ptr(gy), _ptr(gz), _ptr(dpts),
@@ -290,7 +293,7 @@ class Handle:
     def execute_knn_points(self, k, px, py, pz=None):
         px, py, pz = _f64(px), _f64(py), _f64(pz)
         m = px.size
-        z = np.empty(m, dtype=np.float64)
+        z = np.empty(max(1, self.n_fields) * m, dtype=np.float64)
         ss = np.empty(m, dtype=np.float64)
         self._check(self._fn("execute_knn_points")(self._h, int(k), m, _ptr(px), _ptr(py), _ptr(pz),
                                                       _ptr(z), _ptr(ss)), knn=True)
@@ -301,7 +304,7 @@ class Handle:
         nx, ny, nz = gx.size, gy.size, (gz.size if gz is not None else 1)
         if count is None:
             count = nx * ny * nz - first
-        z = np.empty(count, dtype=np.float64)
+        z = np.empty(max(1, self.n_fields) * count, dtype=np.float64)
         ss = np.empty(count, dtype=np.float64)
         self._check(self._fn("execute_knn_grid")(self._h, int(k), nx, ny, nz, _ptr(gx), _ptr(gy), _ptr(gz),
                                                     int(first), int(count), _ptr(z), _ptr(ss)), knn=True)
@@ -362,6 +365,19 @@ class Handle:
         else:
             args = (0, 0, None, None, None)
         self._check(self.lib.kb200_set_device_drift(self._h, 0 if w is None else w.shape[0], _ptr(w), *args))
+
+    def set_values(self, fields):
+        """Value fields for the next set_problem / set_problem_knn (kb200_set_values): fields = (V, n) array, one
+        field per row, or None to krige the problem's own values. The execute methods then return z as V
+        consecutive blocks of the point count."""
+        if fields is None:
+            self._check(self.lib.kb200_set_values(self._h, 0, 0, None))
+            self.n_fields = 0
+            return
+        f = np.ascontiguousarray(fields, dtype=np.float64)      # (V, n) row-major = column-major n x V
+        self.n_fields = 0
+        self._check(self.lib.kb200_set_values(self._h, int(f.shape[0]), int(f.shape[1]), _ptr(f)))
+        self.n_fields = int(f.shape[0])
 
     def experimental_variogram(self, X, values, nlags, geographic=False):
         """Device twin of the pdist binning (core.py:432-505): X = (n, 2|3) ADJUSTED coordinates (or

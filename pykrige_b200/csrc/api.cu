@@ -17,6 +17,7 @@ static const int64_t KB_STAGE_PTS = 1 << 20;   // prediction points per staged o
 #define KB_TILE_COST_32 0.607     // one round of 32-point tiles relative to one round of 64-point tiles (fp64 kernel, N=5000,
 #define KB_TILE_COST_16 0.403     // one H100 80GB HBM3 at 400 W: 5.26 / 3.19 / 2.12 ms per round; scripts/tile_timing.py)
 static const int64_t KB_STAGE_MIN = 1 << 18;   // below this the outputs go straight to the caller's buffers
+#define KB_TN_FIELDS 32   // widest point tile of the value-fields solve kernels (solve.cu: no spills up to 32 points)
 
 struct Src {
     bool grid; int64_t nx, ny, nz;
@@ -63,6 +64,12 @@ struct kb200_ctx {
     PackMap pm{};
     std::vector<double> hx, hy, hz, hval, hdrift;
     double bb_lo[3] = {0, 0, 0}, bb_hi[3] = {0, 0, 0};   // adjusted bounding box of the data
+    // value fields (kb200_set_values): nf columns of nf_n values, column-major; nf = 0: the problem's own values
+    int nf = 0; int64_t nf_n = 0;
+    std::vector<double> hfields;
+    int aux_cols = KB_MAXAUX;  // columns of each of Fz / Hz / Uz in wF: max(KB_MAXAUX, na)
+    int64_t zstride = 0;       // z_out block stride of the fields in the running execute call
+    int pin_blocks = 0;        // capacity of each pinned staging buffer, in blocks of KB_STAGE_PTS doubles
 
     // blob (one allocation): header | consts | ax | ay | az | tiles
     DevBuf blob;
@@ -71,7 +78,7 @@ struct kb200_ctx {
     // factor workspace
     DevBuf wC, wW, wT, wF, wRaw, wFlag;
     // execute workspace
-    DevBuf wPart, wAux, wPts, wOut, wAxes, wDrift, wScratch;
+    DevBuf wPart, wAux, wPts, wOut, wAxes, wDrift, wScratch, wFstage;
     int num_sms = 132;
     // device-evaluated drift terms (kb200_set_device_drift): configuration + the count used by the described problem
     DeviceDrift dd{};
@@ -85,7 +92,7 @@ struct kb200_ctx {
     cudaStream_t hi_stream = nullptr;
     std::vector<cudaEvent_t> fev;
     // knn workspace
-    DevBuf kSorted, kCells;
+    DevBuf kSorted, kCells, kFields;
     DevBuf wVario;            // constructor-side helpers (experimental variogram, statistics)
     DevBuf wTab;              // KB200_VG_TABLE: (value, slope) pairs on the device
     std::vector<double> htab; // ... and on the host (value, slope interleaved), for the covariance shift
@@ -136,7 +143,7 @@ extern "C" void kb200_destroy(kb200_handle h) {
     cudaSetDevice(h->device);
     cudaStreamSynchronize(h->stream);
     for (DevBuf* b : {&h->blob, &h->wC, &h->wW, &h->wT, &h->wF, &h->wRaw, &h->wFlag, &h->wPart, &h->wAux,
-                      &h->wPts, &h->wOut, &h->wAxes, &h->wDrift, &h->wScratch, &h->kSorted, &h->kCells, &h->wVario, &h->wTab,
+                      &h->wPts, &h->wOut, &h->wAxes, &h->wDrift, &h->wScratch, &h->wFstage, &h->kSorted, &h->kCells, &h->kFields, &h->wVario, &h->wTab,
                       &h->wWells, &h->wExt}) b->release();
     for (int i = 0; i < 2; ++i) {
         if (h->pin[i]) cudaFreeHost(h->pin[i]);
@@ -174,6 +181,24 @@ extern "C" int kb200_set_pseudo_inverse(kb200_handle h, int enable) {
     if (!h) return KB200_EBADARG;
     h->pinv = enable ? 1 : 0;
     h->described = false; h->ready = false; h->knn_ready = false; h->factor_live = false;
+    return KB200_OK;
+}
+
+extern "C" int kb200_set_values(kb200_handle h, int n_fields, int64_t n, const double* values) {
+    if (!h) return KB200_EBADARG;
+    h->described = false; h->ready = false; h->knn_ready = false; h->factor_live = false;
+    h->nf = 0; h->nf_n = 0; h->hfields.clear();
+    if (n_fields == 0) return KB200_OK;
+    if (n_fields < 0 || n_fields > KB200_MAX_FIELDS)
+        return fail(h, KB200_EBADARG, "n_fields must be in [0, " + std::to_string(KB200_MAX_FIELDS) + "]");
+    if (n < 1 || n > (1LL << 30) || !values) return fail(h, KB200_EBADARG, "values: n >= 1 rows and a non-NULL array");
+    const size_t cnt = (size_t)n * n_fields;
+    for (size_t i = 0; i < cnt; ++i)
+        if (!std::isfinite(values[i]))
+            return fail(h, KB200_EBADARG, "values must be finite (field " + std::to_string(i / n) + ", row " +
+                        std::to_string(i % n) + ")");
+    h->hfields.assign(values, values + cnt);
+    h->nf = n_fields; h->nf_n = n;
     return KB200_OK;
 }
 
@@ -267,11 +292,20 @@ static int describe(kb200_ctx* h, bool knn_only, int dim, int dtype, int64_t n,
     if (n_dev > n_hd) return fail(h, KB200_EBADARG, "device drift terms (kb200_set_device_drift) exceed the n_hd described drift columns");
     if (n_dev && dim != 2) return fail(h, KB200_EUNSUPPORTED, "point_log / external_Z drift terms are two-dimensional (uk.py)");
     h->n_dev = n_dev;
+    if (h->nf) {
+        if (n != h->nf_n) return fail(h, KB200_EBADARG, "kb200_set_values: the fields have " + std::to_string(h->nf_n) +
+                                      " rows, the problem " + std::to_string(n) + " data points");
+        if (!knn_only && dtype != KB200_F64) return fail(h, KB200_EUNSUPPORTED, "value fields run in float64 only");
+        if (!knn_only && h->pinv) return fail(h, KB200_EUNSUPPORTED, "value fields are not supported with pseudo_inv=True");
+    }
     h->slices = dtype == KB200_F64X ? 6 : dtype == KB200_F64X5 ? 5 : dtype == KB200_F64X4 ? 4 : 0;
 
     const int user_dim = dim;
     h->dim = h->geo ? KB_GEO : dim; h->dtype = dtype; h->n = (int)n; h->n_rl = n_rl; h->n_hd = n_hd;
-    h->K1 = n_rl + n_hd + 1; h->na = h->K1 + 1;
+    // dual rows: K + 1 drift/unbiasedness rows and one zeta row per value field (n + na <= n + 80 stays within
+    // KB_MAXRB row blocks for every n the check above admits)
+    h->K1 = n_rl + n_hd + 1; h->na = h->K1 + (h->nf ? h->nf : 1);
+    h->aux_cols = std::max(KB_MAXAUX, h->na);
     h->vg.model = model;
     h->vg.p0 = need > 0 ? vparams[0] : 0.0; h->vg.p1 = need > 1 ? vparams[1] : 0.0; h->vg.p2 = (need == 3) ? vparams[2] : 0.0;
     h->vg.inv_a = 0.0;
@@ -360,7 +394,7 @@ static int describe(kb200_ctx* h, bool knn_only, int dim, int dtype, int64_t n,
     size_t esz = 8;   // fp64 value, or TF32 hi + lo pair: both 8 bytes per element
     size_t o = 0;
     o += align_up(64 * sizeof(double), 256);
-    h->off_consts = o; o += align_up(512 * sizeof(double), 256);
+    h->off_consts = o; o += align_up((size_t)std::max(512, h->K1 * h->na) * sizeof(double), 256);   // S^-1 | phi_v
     h->off_ax = o; o += align_up((size_t)h->n_pad * 8, 256);
     h->off_ay = o; o += align_up((size_t)h->n_pad * 8, 256);
     h->off_az = o; o += align_up((size_t)h->n_pad * 8, 256);
@@ -384,6 +418,7 @@ extern "C" int kb200_describe_problem(kb200_handle h, int dim, int dtype, int64_
                                       const double* center, const double* aniso,
                                       int model, const double* vparams, int n_vparams,
                                       int exact_values, double eps, int n_rl, int n_hd, const double* drift_data) {
+    if (h && h->nf) return fail(h, KB200_EUNSUPPORTED, "value fields (kb200_set_values) have no factor-blob form");
     return describe(h, false, dim, dtype, n, x, y, z, values, center, aniso, model, vparams, n_vparams,
                     exact_values, eps, n_rl, n_hd, drift_data);
 }
@@ -422,11 +457,14 @@ extern "C" int kb200_set_problem(kb200_handle h, int dim, int dtype, int64_t n,
     const int np = h->n_pad, ld = h->ld, nn = h->n;
     const size_t mat = (size_t)np * ld * sizeof(double);
     CU(h, h->wC.reserve(mat)); CU(h, h->wW.reserve(mat)); CU(h, h->wT.reserve(mat));
-    CU(h, h->wF.reserve((size_t)3 * KB_MAXAUX * np * sizeof(double)));
-    CU(h, h->wRaw.reserve((size_t)(4 + h->n_hd) * nn * sizeof(double)));
+    CU(h, h->wF.reserve((size_t)3 * h->aux_cols * np * sizeof(double)));
+    CU(h, h->wRaw.reserve((size_t)(4 + h->n_hd + h->nf) * nn * sizeof(double)));
     CU(h, h->wFlag.reserve(256));
     double* raw = h->wRaw.as<double>();
     double *rx = raw, *ry = raw + nn, *rz = raw + 2 * (size_t)nn, *rv = raw + 3 * (size_t)nn, *rh = raw + 4 * (size_t)nn;
+    double* rf = rh + (size_t)h->n_hd * nn;          // value fields: nf columns of nn
+    const int nv = h->nf ? h->nf : 1;
+    const double* vals = h->nf ? rf : rv;
     char* blob = h->blob.as<char>();
     double* ax = reinterpret_cast<double*>(blob + h->off_ax);
     double* ay = reinterpret_cast<double*>(blob + h->off_ay);
@@ -441,6 +479,7 @@ extern "C" int kb200_set_problem(kb200_handle h, int dim, int dtype, int64_t n,
     CU(h, cudaMemcpyAsync(rz, h->hz.data(), nn * 8, cudaMemcpyHostToDevice, st));
     CU(h, cudaMemcpyAsync(rv, h->hval.data(), nn * 8, cudaMemcpyHostToDevice, st));
     if (h->n_hd) CU(h, cudaMemcpyAsync(rh, h->hdrift.data(), (size_t)h->n_hd * nn * 8, cudaMemcpyHostToDevice, st));
+    if (h->nf) CU(h, cudaMemcpyAsync(rf, h->hfields.data(), (size_t)h->nf * nn * 8, cudaMemcpyHostToDevice, st));
     CU(h, cudaMemsetAsync(ax, 0, (size_t)np * 8, st));
     CU(h, cudaMemsetAsync(ay, 0, (size_t)np * 8, st));
     CU(h, cudaMemsetAsync(az, 0, (size_t)np * 8, st));
@@ -491,9 +530,9 @@ extern "C" int kb200_set_problem(kb200_handle h, int dim, int dtype, int64_t n,
     }
     h->gform = 0;
     double* Fz = h->wF.as<double>();
-    double* Hz = Fz + (size_t)KB_MAXAUX * np;
-    double* Uz = Hz + (size_t)KB_MAXAUX * np;
-    CU(h, cudaMemsetAsync(consts, 0, 512 * sizeof(double), st));
+    double* Hz = Fz + (size_t)h->aux_cols * np;
+    double* Uz = Hz + (size_t)h->aux_cols * np;
+    CU(h, cudaMemsetAsync(consts, 0, (size_t)std::max(512, h->K1 * h->na) * sizeof(double), st));
     if (h->pinv) {
         // pseudo_inv=True: A^+ of the bordered gamma-form matrix (pinv.cu), then the quadratic-form solve
         const int nt = nn + h->K1;
@@ -536,13 +575,13 @@ extern "C" int kb200_set_problem(kb200_handle h, int dim, int dtype, int64_t n,
         }
         h->gform = 1;
         CU(h, cudaEventRecord(h->ev[5], st));
-        CU(h, kbk_dual_gform(h->wC.as<double>(), ld, nn, np, h->n_rl, h->n_hd, ax, ay, az, h->ds, rh, rv,
+        CU(h, kbk_dual_gform(h->wC.as<double>(), ld, nn, np, h->n_rl, h->n_hd, nv, ax, ay, az, h->ds, rh, vals,
                              Fz, Uz, consts, flag, st, &launches));
         CU(h, kbk_pack_gform(h->wC.as<double>(), ld, nn, np, h->na, Uz, h->pm, blob + h->off_tiles, st)); ++launches;
     } else {
     CU(h, kbk_trtri(h->wC.as<double>(), h->wW.as<double>(), h->wT.as<double>(), ld, np, st, &launches));
     CU(h, cudaEventRecord(h->ev[5], st));
-    CU(h, kbk_dual(h->wW.as<double>(), ld, nn, np, h->n_rl, h->n_hd, ax, ay, az, h->ds, rh, rv,
+    CU(h, kbk_dual(h->wW.as<double>(), ld, nn, np, h->n_rl, h->n_hd, nv, ax, ay, az, h->ds, rh, vals,
                    Fz, Hz, Uz, consts, flag, st, &launches));
     if (h->dtype == KB200_F32) {
         CU(h, kbk_pack_tf32(h->wW.as<double>(), ld, nn, np, h->na, Uz, h->pm, blob + h->off_tiles, st));
@@ -647,6 +686,11 @@ static int launch_solve(kb200_ctx* h, const Src& s, double* d_z, double* d_ss, i
     pp.drift_pts = s.d_drift; pp.drift_stride = s.drift_stride; pp.drift_first = s.drift_first;
     pp.m = s.count; pp.scratch = h->wScratch.as<double>(); pp.gform = h->gform;
     pp.z_out = d_z; pp.ss_out = d_ss;
+    pp.nf = h->nf; pp.zstride = h->zstride;
+    if (h->nf) {
+        CU(h, h->wFstage.reserve((size_t)grid * h->na * tp * sizeof(double)));
+        pp.fstage = h->wFstage.as<double>();
+    }
     pp.rowscale = reinterpret_cast<const double*>(blob + h->off_rowscale);
     if (i8) CU(h, kbk_solve_i8(h->slices, h->dim, pp, grid, st));
     else if (f32) CU(h, kbk_solve_tf32(h->dim, pp, grid, st));
@@ -668,20 +712,22 @@ static int run_solve(kb200_ctx* h, const Src& s, double* d_z, double* d_ss) {
     // fp64 DMMA kernel: full rounds of 64-point tiles over all SMs, then the leftover points as ONE more launch whose tile
     // width minimises rounds x cost: a partial round of 64-point tiles keeps a few SMs busy for a whole tile time
     const long long S = h->num_sms;
+    const int TW = h->nf ? KB_TN_FIELDS : KB_TN;               // widest tile of the kernel variant
     if (const char* e = std::getenv("KB200_TILE")) {           // profiling override: one launch, fixed width
-        const int t = std::atoi(e);
+        const int t = std::min(std::atoi(e), TW);
         if (t == 64 || t == 32 || t == 16) return launch_solve(h, s, d_z, d_ss, t);
     }
-    const long long nt64 = (s.count + KB_TN - 1) / KB_TN;
-    const long long main_pts = std::min<long long>(s.count, (nt64 / S) * S * KB_TN);
+    const long long nt64 = (s.count + TW - 1) / TW;
+    const long long main_pts = std::min<long long>(s.count, (nt64 / S) * S * TW);
     const long long rem = s.count - main_pts;
     if (main_pts > 0) {
         Src m = s; m.count = main_pts;
-        int rc = launch_solve(h, m, d_z, d_ss, KB_TN); if (rc) return rc;
+        int rc = launch_solve(h, m, d_z, d_ss, TW); if (rc) return rc;
     }
     if (rem > 0) {
-        int best = KB_TN; double bc = 1e300;
+        int best = TW; double bc = 1e300;
         for (int tp : {64, 32, 16}) {
+            if (tp > TW) continue;
             const long long nt = (rem + tp - 1) / tp;
             const double c = (double)((nt + S - 1) / S) * tile_cost(tp);
             if (c < bc * 0.999) { bc = c; best = tp; }
@@ -697,17 +743,20 @@ static int run_knn(kb200_ctx* h, int k, const Src& s, double* d_z, double* d_ss,
 // Launch `total` points in chunks and bring (z, ss) to the caller's HOST buffers. Large outputs travel through two
 // pinned staging buffers on a second stream while the next chunk computes; the host drains a buffer into the
 // caller's (pageable) memory while the GPU works. launch(o, m, d_z, d_ss) enqueues points [o, o+m) of the call.
+// With value fields z has nf blocks of `total` (field f at z + f * total), on the device as in the caller's buffer.
 template <class Launch>
 static int run_to_host(kb200_ctx* h, int64_t total, double* z_out, double* ss_out, Launch launch) {
     cudaStream_t st = h->stream;
-    CU(h, h->wOut.reserve((size_t)2 * total * 8));
+    const int nzb = h->nf ? h->nf : 1;               // z blocks; a staging buffer holds nzb + 1 blocks (z ..., ss)
+    h->zstride = total;
+    CU(h, h->wOut.reserve((size_t)(nzb + 1) * total * 8));
     double* dz = h->wOut.as<double>();
-    double* dss = dz + total;
+    double* dss = dz + (size_t)nzb * total;
     CU(h, cudaEventRecord(h->ev[7], st));
     if (total < KB_STAGE_MIN) {
         int rc = launch((int64_t)0, total, dz, dss); if (rc) return rc;
         CU(h, cudaEventRecord(h->ev[8], st));
-        CU(h, cudaMemcpyAsync(z_out, dz, total * 8, cudaMemcpyDeviceToHost, st));
+        CU(h, cudaMemcpyAsync(z_out, dz, (size_t)nzb * total * 8, cudaMemcpyDeviceToHost, st));
         CU(h, cudaMemcpyAsync(ss_out, dss, total * 8, cudaMemcpyDeviceToHost, st));
         CU(h, cudaEventRecord(h->ev[11], st));
         CU(h, cudaStreamSynchronize(st));
@@ -717,10 +766,16 @@ static int run_to_host(kb200_ctx* h, int64_t total, double* z_out, double* ss_ou
     if (!h->copy_stream) {
         CU(h, cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
         for (int i = 0; i < 2; ++i) {
-            CU(h, cudaHostAlloc(&h->pin[i], (size_t)2 * KB_STAGE_PTS * 8, cudaHostAllocDefault));
             CU(h, cudaEventCreateWithFlags(&h->evk[i], cudaEventDisableTiming));
             CU(h, cudaEventCreate(&h->evc[i]));
         }
+    }
+    if (h->pin_blocks < nzb + 1) {
+        for (int i = 0; i < 2; ++i) {
+            if (h->pin[i]) { CU(h, cudaFreeHost(h->pin[i])); h->pin[i] = nullptr; }
+            CU(h, cudaHostAlloc(&h->pin[i], (size_t)(nzb + 1) * KB_STAGE_PTS * 8, cudaHostAllocDefault));
+        }
+        h->pin_blocks = nzb + 1;
     }
     const int64_t nch = (total + KB_STAGE_PTS - 1) / KB_STAGE_PTS;
     auto chunk_len = [&](int64_t c) { return std::min<int64_t>(KB_STAGE_PTS, total - c * KB_STAGE_PTS); };
@@ -729,8 +784,9 @@ static int run_to_host(kb200_ctx* h, int64_t total, double* z_out, double* ss_ou
         CU(h, cudaEventSynchronize(h->evc[b]));
         const double* p = reinterpret_cast<const double*>(h->pin[b]);
         const int64_t m = chunk_len(c);
-        std::memcpy(z_out + c * KB_STAGE_PTS, p, (size_t)m * 8);
-        std::memcpy(ss_out + c * KB_STAGE_PTS, p + KB_STAGE_PTS, (size_t)m * 8);
+        for (int f = 0; f < nzb; ++f)
+            std::memcpy(z_out + (size_t)f * total + c * KB_STAGE_PTS, p + (size_t)f * KB_STAGE_PTS, (size_t)m * 8);
+        std::memcpy(ss_out + c * KB_STAGE_PTS, p + (size_t)nzb * KB_STAGE_PTS, (size_t)m * 8);
         return KB200_OK;
     };
     for (int64_t c = 0; c < nch; ++c) {
@@ -742,8 +798,10 @@ static int run_to_host(kb200_ctx* h, int64_t total, double* z_out, double* ss_ou
         if (c >= 2) { rc = drain(c - 2); if (rc) return rc; }
         double* p = reinterpret_cast<double*>(h->pin[b]);
         CU(h, cudaStreamWaitEvent(h->copy_stream, h->evk[b], 0));
-        CU(h, cudaMemcpyAsync(p, dz + o, (size_t)m * 8, cudaMemcpyDeviceToHost, h->copy_stream));
-        CU(h, cudaMemcpyAsync(p + KB_STAGE_PTS, dss + o, (size_t)m * 8, cudaMemcpyDeviceToHost, h->copy_stream));
+        for (int f = 0; f < nzb; ++f)
+            CU(h, cudaMemcpyAsync(p + (size_t)f * KB_STAGE_PTS, dz + (size_t)f * total + o, (size_t)m * 8,
+                                  cudaMemcpyDeviceToHost, h->copy_stream));
+        CU(h, cudaMemcpyAsync(p + (size_t)nzb * KB_STAGE_PTS, dss + o, (size_t)m * 8, cudaMemcpyDeviceToHost, h->copy_stream));
         CU(h, cudaEventRecord(h->evc[b], h->copy_stream));
     }
     for (int64_t c = std::max<int64_t>(0, nch - 2); c < nch; ++c) { int rc = drain(c); if (rc) return rc; }
@@ -768,6 +826,7 @@ extern "C" int kb200_execute_points_dev(kb200_handle h, int64_t m,
     if (!d_px || !d_py || (h->dim == 3 && !d_pz) || !d_z || !d_ss) return fail(h, KB200_EBADARG, "null pointer");
     if (n_host_drift(h) && !d_drift_pts) return fail(h, KB200_EBADARG, "drift values at the points are required");
     Src s{false, 0, 0, 0, d_px, d_py, d_pz, 0, m, d_drift_pts, m, 0};
+    h->zstride = m;
     CU(h, cudaEventRecord(h->ev[7], h->stream));
     rc = run_solve(h, s, d_z, d_ss); if (rc) return rc;
     CU(h, cudaEventRecord(h->ev[8], h->stream));
@@ -793,6 +852,7 @@ extern "C" int kb200_execute_grid_dev(kb200_handle h, int64_t nx, int64_t ny, in
     if (!d_gx || !d_gy || (h->dim == 3 && !d_gz) || !d_z || !d_ss) return fail(h, KB200_EBADARG, "null pointer");
     if (n_host_drift(h) && !d_drift_pts) return fail(h, KB200_EBADARG, "drift values at the points are required");
     Src s{true, nx, ny, nz, d_gx, d_gy, d_gz, first, count, d_drift_pts, count, 0};
+    h->zstride = count;
     CU(h, cudaEventRecord(h->ev[7], h->stream));
     rc = run_solve(h, s, d_z, d_ss); if (rc) return rc;
     CU(h, cudaEventRecord(h->ev[8], h->stream));
@@ -953,6 +1013,14 @@ extern "C" int kb200_set_problem_knn(kb200_handle h, int dim, int64_t n,
     int* cursor = cell_start + (ncells + 1);
     CU(h, kbk_knn_build(h->dim, nn, ax, ay, az, rv, kp, sx, sy, sz, sv, sorig, cell_of, cell_start, cursor,
                         ncells, st, &launches));
+    if (h->nf) {                                   // value fields, field-major in the cell-sorted order
+        const size_t fb = (size_t)h->nf * nn * sizeof(double);
+        CU(h, h->kFields.reserve(2 * fb));
+        double* raw_f = h->kFields.as<double>() + (size_t)h->nf * nn;
+        CU(h, cudaMemcpyAsync(raw_f, h->hfields.data(), fb, cudaMemcpyHostToDevice, st));
+        CU(h, kbk_knn_sort_fields(nn, h->nf, sorig, raw_f, h->kFields.as<double>(), st)); ++launches;
+        kp.values = h->kFields.as<double>(); kp.nv = h->nf;
+    }
     CU(h, cudaEventRecord(h->ev[2], st));
     CU(h, cudaStreamSynchronize(st));
     h->tm[6] += ev_ms(h->ev[0], h->ev[1]);
@@ -980,7 +1048,7 @@ static int run_knn(kb200_ctx* h, int k, const Src& s, double* d_z, double* d_ss,
     ps.grid = s.grid ? 1 : 0;
     ps.px = s.a; ps.py = s.b; ps.pz = s.c; ps.gx = s.a; ps.gy = s.b; ps.gz = s.c;
     ps.nx = s.nx; ps.ny = s.ny; ps.nz = s.nz; ps.first = s.first;
-    kp.ps = ps; kp.m = s.count; kp.z_out = d_z; kp.ss_out = d_ss; kp.flag = h->wFlag.as<int>();
+    kp.ps = ps; kp.m = s.count; kp.z_out = d_z; kp.ss_out = d_ss; kp.flag = h->wFlag.as<int>(); kp.zstride = h->zstride;
     CU(h, kbk_knn_solve(kp, chol, st));
     h->launches += 1; h->solve_launches += 1;
     return KB200_OK;
@@ -992,7 +1060,7 @@ static int check_knn(kb200_ctx* h, int k) {
     cudaSetDevice(h->device);
     if (k < 2) return fail(h, KB200_EBADARG, "n_closest_points has to be at least two!");
     if (k > h->n) return fail(h, KB200_EBADARG, "n_closest_points exceeds the number of data points");
-    if (kbk_knn_smem_per_warp(k, 0, 1) > 200 * 1024) return fail(h, KB200_EUNSUPPORTED, "n_closest_points too large for the shared-memory local solver");
+    if (kbk_knn_smem_per_warp(k, 0, 1, 1) > 200 * 1024) return fail(h, KB200_EUNSUPPORTED, "n_closest_points too large for the shared-memory local solver");
     return KB200_OK;
 }
 
@@ -1025,6 +1093,7 @@ extern "C" int kb200_execute_knn_grid_dev(kb200_handle h, int k, int64_t nx, int
     if (count == 0) return KB200_OK;
     if (!d_gx || !d_gy || (h->dim == 3 && !d_gz) || !d_z || !d_ss) return fail(h, KB200_EBADARG, "null pointer");
     Src s{true, nx, ny, nz, d_gx, d_gy, d_gz, first, count, nullptr, 0, 0};
+    h->zstride = count;
     int* flag = h->wFlag.as<int>();
     for (int chol = 1; chol >= 0; --chol) {
         CU(h, cudaMemsetAsync(flag, 0, sizeof(int), h->stream));
@@ -1168,6 +1237,7 @@ extern "C" int kb200_group_set_problem(kb200_group g, int dim, int dtype, int64_
                                        int model, const double* vparams, int n_vparams,
                                        int exact_values, double eps, int n_rl, int n_hd, const double* drift_data) {
     if (!g || g->m.empty()) return KB200_EBADARG;
+    for (auto* m : g->m) if (m->nf) return gfail(g, KB200_EUNSUPPORTED, "value fields (kb200_set_values) have no group form");
     // member 0 assembles + factors while the peers describe the problem (allocating their blobs)
     int rc = group_parallel(g, [&](int i) {
         if (i == 0) return kb200_set_problem(g->m[0], dim, dtype, n, x, y, z, values, center, aniso, model, vparams,
@@ -1205,6 +1275,7 @@ extern "C" int kb200_group_set_problem_knn(kb200_group g, int dim, int64_t n,
                                            const double* center, const double* aniso,
                                            int model, const double* vparams, int n_vparams, int exact_values, double eps) {
     if (!g || g->m.empty()) return KB200_EBADARG;
+    for (auto* m : g->m) if (m->nf) return gfail(g, KB200_EUNSUPPORTED, "value fields (kb200_set_values) have no group form");
     // every device builds its own cell grid from the coordinates (1.6-2.4 MB of input; nothing to broadcast)
     return group_parallel(g, [&](int i) {
         return kb200_set_problem_knn(g->m[i], dim, n, x, y, z, values, center, aniso, model, vparams, n_vparams,
@@ -1315,6 +1386,8 @@ extern "C" int kb200_experimental_variogram(kb200_handle h, int dim, int64_t n,
 extern "C" int kb200_statistics(kb200_handle h, double* delta, double* sigma) {
     if (!h || !delta || !sigma) return KB200_EBADARG;
     if (!h->ready) return fail(h, KB200_ESTATE, "no factored problem: call kb200_set_problem first");
+    if (h->nf) return fail(h, KB200_EUNSUPPORTED, "cross-validation statistics belong to the problem's own values, "
+                           "not to kb200_set_values fields");
     if (h->gform) return fail(h, KB200_EUNSUPPORTED, "cross-validation statistics need the positive definite "
                               "covariance form (this problem runs on the general fallback)");
     if (!h->factor_live) return fail(h, KB200_ESTATE, "the Cholesky factor is not on this handle "
@@ -1326,7 +1399,7 @@ extern "C" int kb200_statistics(kb200_handle h, double* delta, double* sigma) {
     const double* ax = reinterpret_cast<double*>(blob + h->off_ax);
     const double* ay = reinterpret_cast<double*>(blob + h->off_ay);
     const double* az = reinterpret_cast<double*>(blob + h->off_az);
-    const double* Hz = h->wF.as<double>() + (size_t)KB_MAXAUX * np;
+    const double* Hz = h->wF.as<double>() + (size_t)h->aux_cols * np;
     const int K = h->n_rl + h->n_hd;                       // Hz row K = L^-1 1, row K+1 = L^-1 Z
     CU(h, h->wVario.reserve((size_t)nn * (2 * sizeof(double) + sizeof(int)) + 256));
     double* d_delta = h->wVario.as<double>();
@@ -1352,11 +1425,12 @@ extern "C" int64_t kb200_debug_fetch(kb200_handle h, int what, double* out, int6
     else if (what == 2) { src = h->wW.p; cnt = mat; }
     else if (what == 3) {
         size_t nU = (size_t)h->na * h->n_pad;
-        size_t total = nU + (size_t)h->K1 * h->K1 + h->K1 + 1;
+        size_t nc = (size_t)h->K1 * h->na;            // Sinv ((K+1)^2) | phi_v ((K+1) per field)
+        size_t total = nU + nc + 1;
         if ((int64_t)total > cap) return KB200_EBADARG;
-        const double* Uz = h->wF.as<double>() + (size_t)2 * KB_MAXAUX * h->n_pad;
+        const double* Uz = h->wF.as<double>() + (size_t)2 * h->aux_cols * h->n_pad;
         if (cudaMemcpy(out, Uz, nU * 8, cudaMemcpyDeviceToHost) != cudaSuccess) return KB200_ECUDA;
-        if (cudaMemcpy(out + nU, h->blob.as<char>() + h->off_consts, ((size_t)h->K1 * h->K1 + h->K1) * 8,
+        if (cudaMemcpy(out + nU, h->blob.as<char>() + h->off_consts, nc * 8,
                        cudaMemcpyDeviceToHost) != cudaSuccess) return KB200_ECUDA;
         out[total - 1] = h->vg.c0;
         return (int64_t)total;

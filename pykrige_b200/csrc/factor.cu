@@ -446,7 +446,8 @@ __global__ void __launch_bounds__(128) trtri_step2_kernel(double* __restrict__ W
 // Regional-linear columns are built on device from the adjusted coordinates
 // (uk.py:877-883, uk3d.py:708-717) with an affine rescale (a change of drift basis,
 // which leaves lambda, z and sigma^2 unchanged because the constant is in the span).
-__global__ void build_fz_kernel(int n, int n_pad, int n_rl, int n_hd,
+// values: nv columns (column-major, stride n) -> Fz columns K+1 .. K+nv
+__global__ void build_fz_kernel(int n, int n_pad, int n_rl, int n_hd, int nv,
                                 const double* __restrict__ ax, const double* __restrict__ ay,
                                 const double* __restrict__ az,
                                 DriftScale ds, const double* __restrict__ hd, const double* __restrict__ values,
@@ -462,7 +463,7 @@ __global__ void build_fz_kernel(int n, int n_pad, int n_rl, int n_hd,
     for (int c = 0; c < n_hd; ++c)
         Fz[(size_t)(n_rl + c) * n_pad + i] = in ? (hd[(size_t)c * n + i] - ds.shift[n_rl + c]) * ds.scale[n_rl + c] : 0.0;
     Fz[(size_t)K * n_pad + i] = in ? 1.0 : 0.0;
-    Fz[(size_t)(K + 1) * n_pad + i] = in ? values[i] : 0.0;
+    for (int v = 0; v < nv; ++v) Fz[(size_t)(K + 1 + v) * n_pad + i] = in ? values[(size_t)v * n + i] : 0.0;
 }
 
 // Hz[i][c] = sum_{k<=i} W[i][k] Fz[k][c]   (one warp per row)
@@ -539,23 +540,22 @@ __global__ void __launch_bounds__(1024) dual_u_kernel(const double* __restrict__
     }
 }
 
-// S = F^T U (K1 x K1), phi = F^T zeta, S^-1 by Gauss-Jordan with partial pivoting.
-// consts layout: [0 .. K1*K1) Sinv, [K1*K1 .. K1*K1+K1) phi. Singular S sets *flag = -1.
-__global__ void __launch_bounds__(256) dual_small_kernel(int n, int n_pad, int K1,
+// S = F^T U (K1 x K1), phi_v = F^T zeta_v (v < nv), S^-1 by Gauss-Jordan with partial pivoting.
+// consts layout: [0 .. K1*K1) Sinv, then phi_0 .. phi_{nv-1}, K1 each. Singular S sets *flag = -1.
+__global__ void __launch_bounds__(256) dual_small_kernel(int n, int n_pad, int K1, int nv,
                                                           const double* __restrict__ Fz, const double* __restrict__ Uz,
                                                           double* __restrict__ consts, int* __restrict__ flag) {
     __shared__ double red[256];
     __shared__ double S[16 * 17];
-    __shared__ double ph[16];
     const int tid = threadIdx.x;
     for (int a = 0; a < K1; ++a) {
-        for (int b = 0; b <= K1; ++b) {     // b == K1 -> zeta column
+        for (int b = 0; b < K1 + nv; ++b) {     // b >= K1 -> zeta columns
             double s = 0.0;
             for (int k = tid; k < n; k += 256) s += Fz[(size_t)a * n_pad + k] * Uz[(size_t)b * n_pad + k];
             red[tid] = s;
             __syncthreads();
             for (int o = 128; o > 0; o >>= 1) { if (tid < o) red[tid] += red[tid + o]; __syncthreads(); }
-            if (tid == 0) { if (b < K1) S[a * 17 + b] = red[0]; else ph[a] = red[0]; }
+            if (tid == 0) { if (b < K1) S[a * 17 + b] = red[0]; else consts[K1 * K1 + (b - K1) * K1 + a] = red[0]; }
             __syncthreads();
         }
     }
@@ -580,10 +580,8 @@ __global__ void __launch_bounds__(256) dual_small_kernel(int n, int n_pad, int K
             }
         }
         if (bad) { if (*flag == 0) *flag = -1; }
-        for (int a = 0; a < K1; ++a) {
+        for (int a = 0; a < K1; ++a)
             for (int b = 0; b < K1; ++b) consts[a * K1 + b] = bad ? 0.0 : M[a][K1 + b];
-            consts[K1 * K1 + a] = ph[a];
-        }
     }
 }
 
@@ -719,22 +717,29 @@ cudaError_t kbk_trtri(const double* L, double* W, double* T1, int ld, int n_pad,
     return cudaGetLastError();
 }
 
-cudaError_t kbk_dual(const double* W, int ld, int n, int n_pad, int n_rl, int n_hd,
+// The dual kernels keep KB_MAXAUX accumulators per thread in registers: more columns (value fields) run as further
+// launches over column chunks of KB_MAXAUX. Every column's arithmetic is the same in whichever chunk it lands.
+cudaError_t kbk_dual(const double* W, int ld, int n, int n_pad, int n_rl, int n_hd, int nv,
                      const double* ax, const double* ay, const double* az, const DriftScale& ds,
                      const double* hd, const double* values,
                      double* Fz, double* Hz, double* Uz, double* consts, int* flag, cudaStream_t st, int* launches) {
-    int K1 = n_rl + n_hd + 1, na = K1 + 1;
-    build_fz_kernel<<<(n_pad + 255) / 256, 256, 0, st>>>(n, n_pad, n_rl, n_hd, ax, ay, az, ds, hd, values, Fz);
-    dual_h_kernel<<<(n + 7) / 8, 256, 0, st>>>(W, ld, n, n_pad, na, Fz, Hz);
-    dual_u_kernel<<<(n_pad + 31) / 32, 1024, 0, st>>>(W, ld, n, n_pad, na, Hz, Uz);
-    dual_small_kernel<<<1, 256, 0, st>>>(n, n_pad, K1, Fz, Uz, consts, flag);
-    *launches += 4;
+    int K1 = n_rl + n_hd + 1, na = K1 + nv;
+    build_fz_kernel<<<(n_pad + 255) / 256, 256, 0, st>>>(n, n_pad, n_rl, n_hd, nv, ax, ay, az, ds, hd, values, Fz);
+    for (int c0 = 0; c0 < na; c0 += KB_MAXAUX) {
+        const int nc = na - c0 < KB_MAXAUX ? na - c0 : KB_MAXAUX;
+        const size_t o = (size_t)c0 * n_pad;
+        dual_h_kernel<<<(n + 7) / 8, 256, 0, st>>>(W, ld, n, n_pad, nc, Fz + o, Hz + o);
+        dual_u_kernel<<<(n_pad + 31) / 32, 1024, 0, st>>>(W, ld, n, n_pad, nc, Hz + o, Uz + o);
+        *launches += 2;
+    }
+    dual_small_kernel<<<1, 256, 0, st>>>(n, n_pad, K1, nv, Fz, Uz, consts, flag);
+    *launches += 2;
     return cudaGetLastError();
 }
 
 cudaError_t kbk_build_fz(int n, int n_pad, int n_rl, int n_hd, const double* ax, const double* ay, const double* az,
                          const DriftScale& ds, const double* hd, const double* values, double* Fz, cudaStream_t st) {
-    build_fz_kernel<<<(n_pad + 255) / 256, 256, 0, st>>>(n, n_pad, n_rl, n_hd, ax, ay, az, ds, hd, values, Fz);
+    build_fz_kernel<<<(n_pad + 255) / 256, 256, 0, st>>>(n, n_pad, n_rl, n_hd, 1, ax, ay, az, ds, hd, values, Fz);
     return cudaGetLastError();
 }
 
@@ -1153,15 +1158,20 @@ cudaError_t kbk_general_inverse(double* C, int ld, int n, int n_pad, void* work,
     return cudaGetLastError();
 }
 
-cudaError_t kbk_dual_gform(const double* G, int ld, int n, int n_pad, int n_rl, int n_hd,
+cudaError_t kbk_dual_gform(const double* G, int ld, int n, int n_pad, int n_rl, int n_hd, int nv,
                            const double* ax, const double* ay, const double* az, const DriftScale& ds,
                            const double* hd, const double* values,
                            double* Fz, double* Uz, double* consts, int* flag, cudaStream_t st, int* launches) {
-    int K1 = n_rl + n_hd + 1, na = K1 + 1;
-    build_fz_kernel<<<(n_pad + 255) / 256, 256, 0, st>>>(n, n_pad, n_rl, n_hd, ax, ay, az, ds, hd, values, Fz);
-    dual_g_kernel<<<(n_pad + 7) / 8, 256, 0, st>>>(G, ld, n, n_pad, na, Fz, Uz);
-    dual_small_kernel<<<1, 256, 0, st>>>(n, n_pad, K1, Fz, Uz, consts, flag);
-    *launches += 3;
+    int K1 = n_rl + n_hd + 1, na = K1 + nv;
+    build_fz_kernel<<<(n_pad + 255) / 256, 256, 0, st>>>(n, n_pad, n_rl, n_hd, nv, ax, ay, az, ds, hd, values, Fz);
+    for (int c0 = 0; c0 < na; c0 += KB_MAXAUX) {      // column chunks, as kbk_dual
+        const int nc = na - c0 < KB_MAXAUX ? na - c0 : KB_MAXAUX;
+        const size_t o = (size_t)c0 * n_pad;
+        dual_g_kernel<<<(n_pad + 7) / 8, 256, 0, st>>>(G, ld, n, n_pad, nc, Fz + o, Uz + o);
+        *launches += 1;
+    }
+    dual_small_kernel<<<1, 256, 0, st>>>(n, n_pad, K1, nv, Fz, Uz, consts, flag);
+    *launches += 2;
     return cudaGetLastError();
 }
 

@@ -45,6 +45,9 @@ struct SolvePtParams {
     const double* rowscale;   // int8-slice path only: 2^(ew_r - 12) per packed row
     double* scratch;          // [grid][ceil(n/16)][16*64]  RHS column blocks in fragment order
     double* z_out; double* ss_out;
+    int nf;                   // value fields (kb200_set_values; fp64 kernel only): the last nf dual rows are zeta_v; the
+    double* fstage;           // row-block epilogue stages all na dual rows in fstage [grid][na][tile points]; phase F writes
+    long long zstride;        // field v of point pj to z_out[v * zstride + pj]
 };
 
 #ifdef __CUDACC__
@@ -89,7 +92,8 @@ __device__ __forceinline__ double kb_ext_sample(const DeviceDrift& dd, double x,
 // adjusted coordinates, uk.py:949-954 / uk3d.py:767-773; point_log + external_Z on the device; the rest from the
 // host-supplied columns), the (K+1)x(K+1) drift solve, and the two outputs. aux[a * astride] = dual-row dot
 // products of this point (rows 0..K: U^T c, row K+1: zeta . c), q = ||W c||^2 (or the quadratic form).
-template <int DIM, typename AuxT>
+// FIELDS (fp64 kernel, P.nf > 0): aux rows K + 1 + v hold zeta_v . c of this point.
+template <int DIM, typename AuxT, bool FIELDS = false>
 __device__ __forceinline__ void kb_finalize_point(const SolvePtParams& P, long long pj, double q,
                                                   const AuxT* aux, int astride) {
     const int K = P.n_rl + P.n_hd, K1 = K + 1;
@@ -137,6 +141,28 @@ __device__ __forceinline__ void kb_finalize_point(const SolvePtParams& P, long l
         return;
     }
     for (int a = 0; a < K1; ++a) r[a] = (double)aux[a * astride] - f[a];
+    if (FIELDS) {
+        // value fields: z_v = zc_v - mu . phi_v with the same mu for every field. Each product and sum is the one of the
+        // single-field branch below, in the same order (mu is recomputed per field: K1^2 flops instead of an array).
+        double rmu = 0.0;
+        for (int a = 0; a < K1; ++a) {
+            double mu = 0.0;
+            for (int b = 0; b < K1; ++b) mu += Sinv[a * K1 + b] * r[b];
+            rmu += r[a] * mu;
+        }
+        P.ss_out[pj] = P.vg.c0 - q + rmu;
+        for (int v = 0; v < P.nf; ++v) {
+            const double* ph = phi + v * K1;
+            double muphi = 0.0;
+            for (int a = 0; a < K1; ++a) {
+                double mu = 0.0;
+                for (int b = 0; b < K1; ++b) mu += Sinv[a * K1 + b] * r[b];
+                muphi += mu * ph[a];
+            }
+            P.z_out[v * P.zstride + pj] = (double)aux[(K1 + v) * astride] - muphi;
+        }
+        return;
+    }
     double rmu = 0.0, muphi = 0.0;
     for (int a = 0; a < K1; ++a) {
         double mu = 0.0;
@@ -157,7 +183,8 @@ cudaError_t kbk_cholesky(double* C, double* W, double* Lstage, int ld, int n_pad
                          cudaStream_t hi, cudaEvent_t* ev, int n_ev, int* launches);   // Lstage: (n_pad/64) x 4096 doubles of scratch;
                                                                                        // hi: high-priority side stream; ev: >= 2*ceil(n_pad/256)+1 events
 cudaError_t kbk_trtri(const double* L, double* W, double* T1, int ld, int n_pad, cudaStream_t st, int* launches);
-cudaError_t kbk_dual(const double* W, int ld, int n, int n_pad, int n_rl, int n_hd,
+// nv value columns (column-major, stride n): Fz / Hz / Uz hold K + 1 + nv columns of stride n_pad each
+cudaError_t kbk_dual(const double* W, int ld, int n, int n_pad, int n_rl, int n_hd, int nv,
                      const double* ax, const double* ay, const double* az, const DriftScale& ds,
                      const double* hd, const double* values,
                      double* Fz, double* Hz, double* Uz, double* consts, int* flag, cudaStream_t st, int* launches);
@@ -169,7 +196,7 @@ cudaError_t kbk_pack(int dtype, const double* W, int ld, int n, int n_pad, int n
 size_t      kbk_general_inverse_workspace_bytes(int n_pad);
 cudaError_t kbk_general_inverse(double* C, int ld, int n, int n_pad, void* work, int* flag, double ptol,
                                 cudaStream_t st, int* launches, int force_scalar);
-cudaError_t kbk_dual_gform(const double* G, int ld, int n, int n_pad, int n_rl, int n_hd,
+cudaError_t kbk_dual_gform(const double* G, int ld, int n, int n_pad, int n_rl, int n_hd, int nv,
                            const double* ax, const double* ay, const double* az, const DriftScale& ds,
                            const double* hd, const double* values,
                            double* Fz, double* Uz, double* consts, int* flag, cudaStream_t st, int* launches);
@@ -218,12 +245,16 @@ struct KnnParams {
     long long m;
     double* z_out; double* ss_out;
     int* flag;                 // singular local system
+    int nv;                    // value columns of `values` (stride n, cell-sorted): 1, or the fields of kb200_set_values
+    long long zstride;         // field v is written to z_out + v * zstride
 };
 cudaError_t kbk_knn_build(int dim, int n, const double* ax, const double* ay, const double* az, const double* values,
                           KnnParams& kp, double* sx, double* sy, double* sz, double* sv, int* sorig,
                           int* cell_of, int* cell_start, int* cursor, int ncells, cudaStream_t st, int* launches);
 cudaError_t kbk_knn_solve(const KnnParams& p, int chol, cudaStream_t st);
-size_t      kbk_knn_smem_per_warp(int k, int chol, int hasz);
+size_t      kbk_knn_smem_per_warp(int k, int chol, int hasz, int nv);
+// dst[v * n + s] = src[v * n + sorig[s]] for v < nv: value fields in the cell-sorted order of the moving window
+cudaError_t kbk_knn_sort_fields(int n, int nv, const int* sorig, const double* src, double* dst, cudaStream_t st);
 
 // variogram.cu: constructor-side kernels (experimental variogram binning, cross-validation residuals)
 cudaError_t kbk_ev_init();

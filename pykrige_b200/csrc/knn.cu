@@ -136,9 +136,10 @@ __global__ void __launch_bounds__(320) knn_solve_kernel(const __grid_constant__ 
     double* base = ksm + (size_t)warp * per_warp_doubles;
     double* A = base;                          // k * S  (aliased by the candidate buffers during the search)
     const int kp = CHOL ? ((k + 7) & ~7) : k;        // padded system size of the tiled Cholesky
-    // tiled Cholesky: nt (nt + 1) / 2 lower tiles + nt augmented tiles + 1 tile for the diagonal inverse, 64 doubles each
-    // — keep in step with kbk_knn_smem_per_warp
-    size_t a_doubles = CHOL ? ((size_t)(kp / 8) * (kp / 8 + 1) / 2 + kp / 8 + 1) * 64 : (size_t)k * S;
+    const int naug = (2 + P.nv + 7) >> 3;            // augmented tile rows: [c ; 1 ; Z_0 .. Z_{nv-1}]
+    // tiled Cholesky: nt (nt + 1) / 2 lower tiles + naug * nt augmented tiles + 1 tile for the diagonal inverse, 64 doubles
+    // each — keep in step with kbk_knn_smem_per_warp
+    size_t a_doubles = CHOL ? ((size_t)(kp / 8) * (kp / 8 + 1) / 2 + (size_t)naug * (kp / 8) + 1) * 64 : (size_t)k * S;
     size_t cand_doubles = KN_CAP + KN_CAP / 2 + KN_SELECT_DOUBLES;   // d2[CAP] doubles + id[CAP] ints + selection scratch
     size_t off = a_doubles > cand_doubles ? a_doubles : cand_doubles;
     // per-neighbour arrays behind the matrix: the tiled Cholesky needs rc, nx, ny, (nz,) nv only (its right-hand sides
@@ -151,7 +152,7 @@ __global__ void __launch_bounds__(320) knn_solve_kernel(const __grid_constant__ 
     double* nx = tailp; double* ny = nx + kp; tailp = ny + kp;
     double* nz = nx;                           // 2-D: never read (kb_dist<2> ignores z)
     if (KB_HASZ(DIM)) { nz = tailp; tailp += kp; }
-    double* nv = tailp;
+    double* ni = tailp;                        // cell-sorted index of each neighbour: field v's value is P.values[v n + i]
     double* cd2 = base;
     int* cid = reinterpret_cast<int*>(base + KN_CAP);
 
@@ -365,7 +366,7 @@ __global__ void __launch_bounds__(320) knn_solve_kernel(const __grid_constant__ 
     }
     for (int t = lane; t < k; t += 32) {
         int i = cid[t];
-        nx[t] = P.ax[i]; ny[t] = P.ay[i]; nv[t] = P.values[i];
+        nx[t] = P.ax[i]; ny[t] = P.ay[i]; ni[t] = (double)i;
         if (KB_HASZ(DIM)) nz[t] = P.az[i];
         // euclidean: the search distance is the kriging distance; geographic: neighbours were ranked by chord
         // length (ok.py:936-960), the kriging distance is the great-circle distance (ok.py:962-969)
@@ -375,7 +376,7 @@ __global__ void __launch_bounds__(320) knn_solve_kernel(const __grid_constant__ 
         if (!CHOL) { cv[t] = c; r1[t] = 1.0; }
     }
     for (int t = k + lane; t < kp; t += 32) {          // identity padding of the blocked system
-        nx[t] = 0.0; ny[t] = 0.0; nv[t] = 0.0; rc[t] = 0.0;
+        nx[t] = 0.0; ny[t] = 0.0; ni[t] = -1.0; rc[t] = 0.0;
         if (KB_HASZ(DIM)) nz[t] = 0.0;
         if (!CHOL) { cv[t] = 0.0; r1[t] = 0.0; }
     }
@@ -392,9 +393,11 @@ __global__ void __launch_bounds__(320) knn_solve_kernel(const __grid_constant__ 
         //     mu = (y_1.y_c - 1) / (y_1.y_1),  z = y_c.y_Z - mu y_1.y_Z,  sigma^2 = c0 - (y_c.y_c - mu y_1.y_c) - mu.
         // Per 8-column step: potf2 + inverse of the diagonal tile in registers (warp shuffles inside groups of 8 lanes),
         // panel tiles X <- X Winv^T and trailing tiles C_ij -= L_ip L_jp^T as DMMAs (2 per tile).
-        const int nt = kp >> 3;                       // tile rows of the covariance block; tile row nt = the augmented rows
-#define KN_T(i, j) (A + ((size_t)(i) * ((i) + 1) / 2 + (j)) * 64)
-        double* Wt = A + ((size_t)nt * (nt + 1) / 2 + nt) * 64;          // inverse of the current diagonal tile
+        // With value fields the augmented rows continue [c ; 1 ; Z_0 ; Z_1 ; ...] over naug tile rows nt .. nt + naug - 1;
+        // every row goes through the same per-row arithmetic, so field v's y_Z does not depend on nv.
+        const int nt = kp >> 3;                       // tile rows of the covariance block; tile rows >= nt = the augmented rows
+#define KN_T(i, j) (A + ((i) < nt ? (size_t)(i) * ((i) + 1) / 2 + (j) : (size_t)nt * (nt + 1) / 2 + (size_t)((i) - nt) * nt + (j)) * 64)
+        double* Wt = A + ((size_t)nt * (nt + 1) / 2 + (size_t)naug * nt) * 64;   // inverse of the current diagonal tile
         const int fr = lane >> 2, fq = lane & 3;
         // assembly: lane <-> (row fr, columns fq and 4 + fq) of every tile; two tiles (four independent sqrt/exp chains)
         // per iteration: the evaluation is latency-bound with 8 warps per SM
@@ -422,15 +425,16 @@ __global__ void __launch_bounds__(320) knn_solve_kernel(const __grid_constant__ 
                 if (tj + 1 <= ti) { T[64 + lane] = v[2]; T[96 + lane] = v[3]; }     // tile (ti, tj + 1) follows (ti, tj)
             }
         }
-        for (int tj = 0; tj < nt; ++tj) {             // augmented rows: 0 = c, 1 = ones, 2 = Z (rows 3..7 zero)
-            double* T = KN_T(nt, tj);
+        for (int ta = 0; ta < naug * nt; ++ta) {      // augmented rows: 0 = c, 1 = ones, 2 + v = Z_v (the rest zero)
+            const int ar = (ta / nt) * 8 + fr, tj = ta % nt;
+            double* T = KN_T(nt + ta / nt, tj);
 #pragma unroll
             for (int half = 0; half < 2; ++half) {
                 const int t = tj * 8 + half * 4 + fq;
                 double v = 0.0;
-                if (fr == 0) v = rc[t];
-                else if (fr == 1) v = (t < k) ? 1.0 : 0.0;
-                else if (fr == 2) v = nv[t];
+                if (ar == 0) v = rc[t];
+                else if (ar == 1) v = (t < k) ? 1.0 : 0.0;
+                else if (ar < 2 + P.nv && t < k) v = P.values[(size_t)(ar - 2) * P.n + (int)ni[t]];
                 T[half * 32 + lane] = v;
             }
         }
@@ -474,10 +478,10 @@ __global__ void __launch_bounds__(320) knn_solve_kernel(const __grid_constant__ 
                 Wt[(gr >> 2) * 32 + (2 * gg + 1) * 4 + (gr & 3)] = v1;
             }
             __syncwarp();
-            // ---- panel: X(i, p) <- X Winv^T for the tile rows below (incl. the augmented row) ----
+            // ---- panel: X(i, p) <- X Winv^T for the tile rows below (incl. the augmented rows) ----
             {
                 const double wb0 = Wt[lane], wb1 = Wt[32 + lane];
-                for (int i = ps + 1; i <= nt; ++i) {
+                for (int i = ps + 1; i < nt + naug; ++i) {
                     double* T = KN_T(i, ps);
                     const double a0 = T[lane], a1 = T[32 + lane];
                     double c0 = 0.0, c1 = 0.0;
@@ -488,9 +492,9 @@ __global__ void __launch_bounds__(320) knn_solve_kernel(const __grid_constant__ 
                 }
             }
             __syncwarp();
-            // ---- trailing update: C(i, j) -= L(i, p) L(j, p)^T,  p < j <= i  (augmented row: j < nt) ----
+            // ---- trailing update: C(i, j) -= L(i, p) L(j, p)^T,  p < j <= i  (augmented rows: j < nt) ----
             // two column tiles per iteration: independent accumulator chains hide the DMMA / LDS latency
-            for (int i = ps + 1; i <= nt; ++i) {
+            for (int i = ps + 1; i < nt + naug; ++i) {
                 const double* Li = KN_T(i, ps);
                 const double a0 = -Li[lane], a1 = -Li[32 + lane];
                 const int jend = i < nt ? i : nt - 1;
@@ -521,26 +525,37 @@ __global__ void __launch_bounds__(320) knn_solve_kernel(const __grid_constant__ 
             __syncwarp();
         }
         if (notpd) {
-            if (lane == 0) { atomicMax(P.flag, 2); P.z_out[p] = 0.0; P.ss_out[p] = 0.0; }
+            if (lane == 0) {
+                atomicMax(P.flag, 2); P.ss_out[p] = 0.0;
+                for (int v = 0; v < P.nv; ++v) P.z_out[p + v * P.zstride] = 0.0;
+            }
             return;
         }
         // ---- bordered-system identities from the augmented rows ----
-        double s11 = 0.0, s1c = 0.0, scc = 0.0, s1z = 0.0, scz = 0.0;
+        double s11 = 0.0, s1c = 0.0, scc = 0.0;
         for (int t = lane; t < kp; t += 32) {
             const double* T = KN_T(nt, t >> 3) + ((t & 7) >> 2) * 32 + (t & 3);
-            const double yc = T[0], y1 = T[4], yz = T[8];
+            const double yc = T[0], y1 = T[4];
             s11 = fma(y1, y1, s11); s1c = fma(y1, yc, s1c); scc = fma(yc, yc, scc);
-            s1z = fma(y1, yz, s1z); scz = fma(yc, yz, scz);
         }
         for (int o = 16; o > 0; o >>= 1) {
             s11 += __shfl_xor_sync(0xffffffffu, s11, o); s1c += __shfl_xor_sync(0xffffffffu, s1c, o);
-            scc += __shfl_xor_sync(0xffffffffu, scc, o); s1z += __shfl_xor_sync(0xffffffffu, s1z, o);
-            scz += __shfl_xor_sync(0xffffffffu, scz, o);
+            scc += __shfl_xor_sync(0xffffffffu, scc, o);
         }
-        if (lane == 0) {
-            const double mu = (s1c - 1.0) / s11;
-            P.z_out[p] = scz - mu * s1z;                       // ok.py:755
-            P.ss_out[p] = vg.c0 - (scc - mu * s1c) - mu;       // ok.py:756 (= -x.b) in covariance form
+        const double mu = (s1c - 1.0) / s11;
+        if (lane == 0) P.ss_out[p] = vg.c0 - (scc - mu * s1c) - mu;       // ok.py:756 (= -x.b) in covariance form
+        for (int v = 0; v < P.nv; ++v) {
+            const int ar = 2 + v;                      // augmented row of field v
+            double s1z = 0.0, scz = 0.0;
+            for (int t = lane; t < kp; t += 32) {
+                const double* T = KN_T(nt, t >> 3) + ((t & 7) >> 2) * 32 + (t & 3);
+                const double yc = T[0], y1 = T[4], yz = KN_T(nt + (ar >> 3), t >> 3)[((t & 7) >> 2) * 32 + (ar & 7) * 4 + (t & 3)];
+                s1z = fma(y1, yz, s1z); scz = fma(yc, yz, scz);
+            }
+            for (int o = 16; o > 0; o >>= 1) {
+                s1z += __shfl_xor_sync(0xffffffffu, s1z, o); scz += __shfl_xor_sync(0xffffffffu, scz, o);
+            }
+            if (lane == 0) P.z_out[p + v * P.zstride] = scz - mu * s1z;                       // ok.py:755
         }
         return;
 #undef KN_T
@@ -609,7 +624,10 @@ __global__ void __launch_bounds__(320) knn_solve_kernel(const __grid_constant__ 
         __syncwarp();
     }
     if (singular) {
-        if (lane == 0) { atomicMax(P.flag, 1); P.z_out[p] = 0.0; P.ss_out[p] = 0.0; }
+        if (lane == 0) {
+            atomicMax(P.flag, 1); P.ss_out[p] = 0.0;
+            for (int v = 0; v < P.nv; ++v) P.z_out[p + v * P.zstride] = 0.0;
+        }
         return;
     }
     // back substitution U x = y for both right-hand sides
@@ -631,32 +649,50 @@ __global__ void __launch_bounds__(320) knn_solve_kernel(const __grid_constant__ 
     for (int t = lane; t < k; t += 32) { s1 += r1[t]; sc += rc[t]; }
     for (int o = 16; o > 0; o >>= 1) { s1 += __shfl_xor_sync(0xffffffffu, s1, o); sc += __shfl_xor_sync(0xffffffffu, sc, o); }
     const double mu = (sc - 1.0) / s1;
-    double zz = 0.0, lc = 0.0;
+    double lc = 0.0;
     for (int t = lane; t < k; t += 32) {
         double lam = rc[t] - mu * r1[t];
-        zz += lam * nv[t];
         lc += lam * cv[t];
     }
-    for (int o = 16; o > 0; o >>= 1) { zz += __shfl_xor_sync(0xffffffffu, zz, o); lc += __shfl_xor_sync(0xffffffffu, lc, o); }
-    if (lane == 0) {
-        P.z_out[p] = zz;                       // ok.py:755
-        P.ss_out[p] = vg.c0 - lc - mu;       // ok.py:756 (= -x.b) in covariance form
+    for (int o = 16; o > 0; o >>= 1) lc += __shfl_xor_sync(0xffffffffu, lc, o);
+    if (lane == 0) P.ss_out[p] = vg.c0 - lc - mu;       // ok.py:756 (= -x.b) in covariance form
+    for (int v = 0; v < P.nv; ++v) {                    // the same weights for every field
+        double zz = 0.0;
+        for (int t = lane; t < k; t += 32) {
+            double lam = rc[t] - mu * r1[t];
+            zz += lam * P.values[(size_t)v * P.n + (int)ni[t]];
+        }
+        for (int o = 16; o > 0; o >>= 1) zz += __shfl_xor_sync(0xffffffffu, zz, o);
+        if (lane == 0) P.z_out[p + v * P.zstride] = zz;                       // ok.py:755
     }
 }
 
 // ---- host side -------------------------------------------------------------
-size_t kbk_knn_smem_per_warp(int k, int chol, int hasz) {
+size_t kbk_knn_smem_per_warp(int k, int chol, int hasz, int nv) {
     size_t S = (size_t)(k | 1);
     size_t kp = chol ? (size_t)((k + 7) & ~7) : (size_t)k;
-    size_t nt = kp / 8;
-    size_t a = chol ? (nt * (nt + 1) / 2 + nt + 1) * 64 : (size_t)k * S, c = KN_CAP + KN_CAP / 2 + KN_SELECT_DOUBLES;
-    const size_t tail = chol ? (hasz ? 5 : 4) : 7;      // rc, nx, ny, (nz,) nv  |  + r1, cv for the LU path
+    size_t nt = kp / 8, naug = (size_t)(2 + nv + 7) / 8;
+    size_t a = chol ? (nt * (nt + 1) / 2 + naug * nt + 1) * 64 : (size_t)k * S, c = KN_CAP + KN_CAP / 2 + KN_SELECT_DOUBLES;
+    const size_t tail = chol ? (hasz ? 5 : 4) : 7;      // rc, nx, ny, (nz,) ni  |  + r1, cv for the LU path
     return ((a > c ? a : c) + tail * kp + 2) * sizeof(double);
+}
+
+__global__ void knn_sort_fields_kernel(int n, int nv, const int* __restrict__ sorig, const double* __restrict__ src,
+                                       double* __restrict__ dst) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n) return;
+    const int i = sorig[s];
+    for (int v = 0; v < nv; ++v) dst[(size_t)v * n + s] = src[(size_t)v * n + i];
+}
+
+cudaError_t kbk_knn_sort_fields(int n, int nv, const int* sorig, const double* src, double* dst, cudaStream_t st) {
+    knn_sort_fields_kernel<<<(n + 255) / 256, 256, 0, st>>>(n, nv, sorig, src, dst);
+    return cudaGetLastError();
 }
 
 template <int DIM, bool CHOL>
 static cudaError_t knn_launch_dim(const KnnParams& p, cudaStream_t st) {
-    size_t per = kbk_knn_smem_per_warp(p.k, CHOL ? 1 : 0, KB_HASZ(DIM) ? 1 : 0);
+    size_t per = kbk_knn_smem_per_warp(p.k, CHOL ? 1 : 0, KB_HASZ(DIM) ? 1 : 0, p.nv);
     int wpc = (int)std::min<size_t>(10, (size_t)(226 * 1024) / per);   // as many points in flight per SM as fit (<= 320 threads; 227 KB minus the static 1 KB)
     if (wpc < 1) return cudaErrorInvalidValue;
     size_t smem = per * wpc;
@@ -694,6 +730,6 @@ cudaError_t kbk_knn_build(int dim, int n, const double* ax, const double* ay, co
     knn_scatter_kernel<<<g, 256, 0, st>>>(n, cell_of, cell_start, cursor, ax, ay, az, values, sx, sy, sz, sv, sorig);
     knn_cellsort_kernel<<<(ncells + 255) / 256, 256, 0, st>>>(ncells, cell_start, sx, sy, sz, sv, sorig);
     *launches += 4;
-    kp.ax = sx; kp.ay = sy; kp.az = sz; kp.values = sv; kp.sorig = sorig; kp.cell_start = cell_start;
+    kp.ax = sx; kp.ay = sy; kp.az = sz; kp.values = sv; kp.sorig = sorig; kp.cell_start = cell_start; kp.nv = 1;
     return cudaGetLastError();
 }

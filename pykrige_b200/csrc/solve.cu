@@ -114,7 +114,9 @@ __device__ __forceinline__ int pt_reduce_scatter_index(int i, int lane) {
 // the persistent CTAs (one per SM) busy for a whole tile time (1953 tiles on 132 SMs = 14.8 rounds at 125 000 points per
 // GPU); as narrow tiles they spread over all SMs and a tile costs little more than streaming W once. The per-point arithmetic
 // does not depend on NT (tests/test_parity_gpu.py::test_tile_width_is_invisible).
-template <int DIM, int MODEL, int NT>
+// FIELDS (kb200_set_values): the dual rows are K + 1 + V rows, staged per CTA in global memory (P.fstage) instead of
+// shared memory; a separate instantiation, so that the single-field kernels keep their code and registers.
+template <int DIM, int MODEL, int NT, bool FIELDS>
 __global__ void __launch_bounds__(PT_THREADS, 1) solve_kernel_pt(const __grid_constant__ SolvePtParams P) {
     constexpr int TN = NT * 8;                                          // points per tile
     extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -295,7 +297,10 @@ __global__ void __launch_bounds__(PT_THREADS, 1) solve_kernel_pt(const __grid_co
                             }
                         } else {
                             if (r < P.n + P.na) {
-                                double* ao = auxs + (r - P.n) * TN + 2 * (lane & 3);
+                                // FIELDS: the K + 1 + V dual rows do not fit in shared memory; they go to this CTA's rows
+                                // of the global staging buffer, which phase F reads back after the barrier
+                                double* ao = (FIELDS ? P.fstage + (int)(blockIdx.x * P.na * TN) : auxs) + (r - P.n) * TN +
+                                             2 * (lane & 3);
 #pragma unroll
                                 for (int nt = 0; nt < NT; ++nt) {
                                     ao[nt * 8] = acc[q][nt][2 * h];
@@ -329,7 +334,10 @@ __global__ void __launch_bounds__(PT_THREADS, 1) solve_kernel_pt(const __grid_co
                 double q = 0.0;
 #pragma unroll
                 for (int w = 0; w < 8; ++w) q += qred[w * TN + tid];     // fixed order: deterministic
-                kb_finalize_point<DIM, double>(P, pj, q, auxs + tid, TN);
+                if constexpr (FIELDS)
+                    kb_finalize_point<DIM, double, true>(P, pj, q, P.fstage + (int)(blockIdx.x * P.na * TN) + tid, TN);
+                else
+                    kb_finalize_point<DIM, double>(P, pj, q, auxs + tid, TN);
             }
         }
         __syncthreads();      // qred / auxs / scratch are re-used by the next tile
@@ -345,14 +353,22 @@ size_t kbk_solve_pt_scratch_doubles(int n, int grid) {
 }
 
 
+// The fields kernels run 32- and 16-point tiles only: with 64-point tiles the global staging of the dual rows costs the
+// 64-point kernel its last registers (ptxas spills), so the widest fields tile is NT = 4 (KB_TN_FIELDS in api.cu).
+template <int DIM, int MODEL, bool FIELDS>
+static cudaError_t solve_set_attr_f() {
+    constexpr int NT8 = FIELDS ? 4 : 8;
+    KB_CUDA_OK(cudaFuncSetAttribute(solve_kernel_pt<DIM, MODEL, NT8, FIELDS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    (int)solve_smem_pt()));
+    KB_CUDA_OK(cudaFuncSetAttribute(solve_kernel_pt<DIM, MODEL, 4, FIELDS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    (int)solve_smem_pt()));
+    return cudaFuncSetAttribute(solve_kernel_pt<DIM, MODEL, 2, FIELDS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                (int)solve_smem_pt());
+}
 template <int DIM, int MODEL>
 static cudaError_t solve_set_attr() {
-    KB_CUDA_OK(cudaFuncSetAttribute(solve_kernel_pt<DIM, MODEL, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)solve_smem_pt()));
-    KB_CUDA_OK(cudaFuncSetAttribute(solve_kernel_pt<DIM, MODEL, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)solve_smem_pt()));
-    return cudaFuncSetAttribute(solve_kernel_pt<DIM, MODEL, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)solve_smem_pt());
+    KB_CUDA_OK((solve_set_attr_f<DIM, MODEL, false>()));
+    return solve_set_attr_f<DIM, MODEL, true>();
 }
 
 cudaError_t kbk_solve_init() {
@@ -363,13 +379,15 @@ cudaError_t kbk_solve_init() {
     return cudaSuccess;
 }
 
-template <int DIM>
+template <int DIM, bool FIELDS>
 static cudaError_t solve_pt_dim(const SolvePtParams& p, int grid, int tile_points, cudaStream_t st) {
     size_t sm = solve_smem_pt();
+    constexpr int NT8 = FIELDS ? 4 : 8;
+    if (FIELDS && tile_points == 64) return cudaErrorInvalidValue;
     switch (p.vg.model) {
-#define KB_CASE(M) case M: if (tile_points == 16) solve_kernel_pt<DIM, M, 2><<<grid, PT_THREADS, sm, st>>>(p); \
-                           else if (tile_points == 32) solve_kernel_pt<DIM, M, 4><<<grid, PT_THREADS, sm, st>>>(p); \
-                           else solve_kernel_pt<DIM, M, 8><<<grid, PT_THREADS, sm, st>>>(p); break;
+#define KB_CASE(M) case M: if (tile_points == 16) solve_kernel_pt<DIM, M, 2, FIELDS><<<grid, PT_THREADS, sm, st>>>(p); \
+                           else if (tile_points == 32) solve_kernel_pt<DIM, M, 4, FIELDS><<<grid, PT_THREADS, sm, st>>>(p); \
+                           else solve_kernel_pt<DIM, M, NT8, FIELDS><<<grid, PT_THREADS, sm, st>>>(p); break;
         KB_CASE(KB200_VG_LINEAR) KB_CASE(KB200_VG_POWER) KB_CASE(KB200_VG_GAUSSIAN)
         KB_CASE(KB200_VG_EXPONENTIAL) KB_CASE(KB200_VG_SPHERICAL) KB_CASE(KB200_VG_HOLE_EFFECT) KB_CASE(KB200_VG_TABLE)
 #undef KB_CASE
@@ -380,7 +398,11 @@ static cudaError_t solve_pt_dim(const SolvePtParams& p, int grid, int tile_point
 
 cudaError_t kbk_solve_pt(int dim, const SolvePtParams& p, int grid, int tile_points, cudaStream_t st) {
     if (tile_points != 64 && tile_points != 32 && tile_points != 16) return cudaErrorInvalidValue;
-    if (dim == KB_GEO) return solve_pt_dim<KB_GEO>(p, grid, tile_points, st);
-    return dim == 2 ? solve_pt_dim<2>(p, grid, tile_points, st) : solve_pt_dim<3>(p, grid, tile_points, st);
+    if (p.nf) {
+        if (dim == KB_GEO) return solve_pt_dim<KB_GEO, true>(p, grid, tile_points, st);
+        return dim == 2 ? solve_pt_dim<2, true>(p, grid, tile_points, st) : solve_pt_dim<3, true>(p, grid, tile_points, st);
+    }
+    if (dim == KB_GEO) return solve_pt_dim<KB_GEO, false>(p, grid, tile_points, st);
+    return dim == 2 ? solve_pt_dim<2, false>(p, grid, tile_points, st) : solve_pt_dim<3, false>(p, grid, tile_points, st);
 }
 

@@ -25,7 +25,7 @@ class OrdinaryKriging(Krige2DMixin, KrigeBase):
                              statistics="eager" if enable_statistics else "off")
 
     def execute(self, style, xpoints, ypoints, mask=None, backend="cuda", n_closest_points=None, dtype="float64",
-                n_gpus=None):
+                n_gpus=None, values=None):
         """Calculates a kriged grid and the associated variance (ok.py:760-1020).
 
         ``backend='cuda'`` is the only backend of this package. ``style``, ``mask`` and
@@ -33,6 +33,14 @@ class OrdinaryKriging(Krige2DMixin, KrigeBase):
         ``n_gpus=G`` shards the prediction points over G GPUs of this box from this one host thread.
         Returns ``(zvalues, sigmasq)`` shaped ``(ny, nx)`` for 'grid'/'masked' (masked arrays
         for 'masked') or ``(n,)`` for 'points'.
+
+        ``values`` (shape ``(N, V)``, row i for data point i of the constructor) kriges V value fields with this
+        object's variogram, anisotropy, drift terms, ``exact_values`` and coordinate type through one factorisation;
+        the constructor's values are neither used nor changed, and the variogram is never refitted to ``values``.
+        ``zvalues`` then gets a leading field axis (``(V, ...)``; for 'masked' the mask is broadcast over it) and
+        ``sigmasq`` keeps its shape, since it does not depend on the values. A 1-D ``values`` of shape ``(N,)``
+        returns the usual shapes. float64 only, one GPU, not with ``pseudo_inv=True`` on the global path. Above
+        ``KB200_MAX_FIELDS`` (64) fields the call runs in chunks of 64, each with its own factorisation.
         """
         if self.verbose:
             print("Executing Ordinary Kriging...\n")
@@ -42,6 +50,9 @@ class OrdinaryKriging(Krige2DMixin, KrigeBase):
             raise ValueError("n_closest_points has to be at least two!")
         axes, sizes, flat_mask = self._prepare_points(style, (xpoints, ypoints), mask)
         self._check_backend(backend, "2D ordinary kriging")
+        fields, one = self._check_values(values, dtype, n_closest_points, n_gpus)
         zvalues, sigmasq = self._run_cuda(style, axes, flat_mask, n_closest_points=n_closest_points, dtype=dtype,
-                                          n_gpus=n_gpus)
+                                          n_gpus=n_gpus, **self._fields_kw(fields))
+        if one:
+            zvalues = zvalues[0]
         return self._shape_output(style, zvalues, sigmasq, sizes, flat_mask)

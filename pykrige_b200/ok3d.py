@@ -151,15 +151,27 @@ class OrdinaryKriging3D(_Krige3DMixin, KrigeBase):
                              pseudo_inv, pseudo_inv_type)
 
     def execute(self, style, xpoints, ypoints, zpoints, mask=None, backend="cuda", n_closest_points=None,
-                dtype="float64", n_gpus=None):
+                dtype="float64", n_gpus=None, values=None):
         """Calculates a kriged 3-D grid and the associated variance (ok3d.py:735-932); ``backend='cuda'``.
-        Output shape (nz, ny, nx) for 'grid'/'masked', (n,) for 'points'."""
+        Output shape (nz, ny, nx) for 'grid'/'masked', (n,) for 'points'.
+
+        ``values`` (shape ``(N, V)``, row i for data point i of the constructor) kriges V value fields with this
+        object's variogram, anisotropy, drift terms, ``exact_values`` and coordinate type through one factorisation;
+        the constructor's values are neither used nor changed, and the variogram is never refitted to ``values``.
+        ``kvalues`` then gets a leading field axis (``(V, ...)``; for 'masked' the mask is broadcast over it) and
+        ``sigmasq`` keeps its shape, since it does not depend on the values. A 1-D ``values`` of shape ``(N,)``
+        returns the usual shapes. float64 only, one GPU, not with ``pseudo_inv=True`` on the global path. Above
+        ``KB200_MAX_FIELDS`` (64) fields the call runs in chunks of 64, each with its own factorisation.
+        """
         if self.verbose:
             print("Executing Ordinary Kriging...\n")
         axes, sizes, flat_mask = self._prepare_points(style, (xpoints, ypoints, zpoints), mask)
         if n_closest_points is not None and n_closest_points <= 1:
             raise ValueError("n_closest_points has to be at least two!")
         self._check_backend(backend, "3D ordinary kriging")
+        fields, one = self._check_values(values, dtype, n_closest_points, n_gpus)
         kvalues, sigmasq = self._run_cuda(style, axes, flat_mask, n_closest_points=n_closest_points, dtype=dtype,
-                                          n_gpus=n_gpus)
+                                          n_gpus=n_gpus, **self._fields_kw(fields))
+        if one:
+            kvalues = kvalues[0]
         return self._shape_output(style, kvalues, sigmasq, sizes, flat_mask)

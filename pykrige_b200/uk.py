@@ -196,11 +196,20 @@ class UniversalKriging(Krige2DMixin, KrigeBase):
         h.set_device_drift(wells, ext)
 
     def execute(self, style, xpoints, ypoints, mask=None, backend="cuda", specified_drift_arrays=None,
-                dtype="float64", n_gpus=None):
+                dtype="float64", n_gpus=None, values=None):
         """Calculates a kriged grid and the associated variance (uk.py:1090-1328); ``backend='cuda'``.
         point_log and external_Z drift terms are evaluated at the prediction points on the device
         (uk.py:955-971, bilinear sampler uk.py:512-628); 'specified' and 'functional' terms are host
-        arrays / host callables by definition and are shipped as columns."""
+        arrays / host callables by definition and are shipped as columns.
+
+        ``values`` (shape ``(N, V)``, row i for data point i of the constructor) kriges V value fields with this
+        object's variogram, anisotropy, drift terms, ``exact_values`` and coordinate type through one factorisation;
+        the constructor's values are neither used nor changed, and the variogram is never refitted to ``values``.
+        ``zvalues`` then gets a leading field axis (``(V, ...)``; for 'masked' the mask is broadcast over it) and
+        ``sigmasq`` keeps its shape, since it does not depend on the values. A 1-D ``values`` of shape ``(N,)``
+        returns the usual shapes. float64 only, one GPU, not with ``pseudo_inv=True`` on the global path. Above
+        ``KB200_MAX_FIELDS`` (64) fields the call runs in chunks of 64, each with its own factorisation.
+        """
         if self.verbose:
             print("Executing Universal Kriging...\n")
         axes, sizes, flat_mask = self._prepare_points(style, (xpoints, ypoints), mask)
@@ -230,5 +239,9 @@ class UniversalKriging(Krige2DMixin, KrigeBase):
                         cols.append(np.asarray(func(xa, ya), dtype=float) * np.ones(xa.shape))
                 return np.ascontiguousarray(np.vstack(cols), dtype=np.float64)
 
-        zvalues, sigmasq = self._run_cuda(style, axes, flat_mask, drift_at=drift_at, dtype=dtype, n_gpus=n_gpus)
+        fields, one = self._check_values(values, dtype, None, n_gpus)
+        zvalues, sigmasq = self._run_cuda(style, axes, flat_mask, drift_at=drift_at, dtype=dtype, n_gpus=n_gpus,
+                                          **self._fields_kw(fields))
+        if one:
+            zvalues = zvalues[0]
         return self._shape_output(style, zvalues, sigmasq, sizes, flat_mask)

@@ -75,8 +75,17 @@ class UniversalKriging3D(_Krige3DMixin, KrigeBase):
         return (3 if self.regional_linear_drift else 0), cols
 
     def execute(self, style, xpoints, ypoints, zpoints, mask=None, backend="cuda", specified_drift_arrays=None,
-                dtype="float64", n_gpus=None):
-        """Calculates a kriged 3-D grid and the associated variance (uk3d.py:877-1146); ``backend='cuda'``."""
+                dtype="float64", n_gpus=None, values=None):
+        """Calculates a kriged 3-D grid and the associated variance (uk3d.py:877-1146); ``backend='cuda'``.
+
+        ``values`` (shape ``(N, V)``, row i for data point i of the constructor) kriges V value fields with this
+        object's variogram, anisotropy, drift terms, ``exact_values`` and coordinate type through one factorisation;
+        the constructor's values are neither used nor changed, and the variogram is never refitted to ``values``.
+        ``kvalues`` then gets a leading field axis (``(V, ...)``; for 'masked' the mask is broadcast over it) and
+        ``sigmasq`` keeps its shape, since it does not depend on the values. A 1-D ``values`` of shape ``(N,)``
+        returns the usual shapes. float64 only, one GPU, not with ``pseudo_inv=True`` on the global path. Above
+        ``KB200_MAX_FIELDS`` (64) fields the call runs in chunks of 64, each with its own factorisation.
+        """
         if self.verbose:
             print("Executing Universal Kriging...\n")
         axes, sizes, flat_mask = self._prepare_points(style, (xpoints, ypoints, zpoints), mask)
@@ -102,5 +111,9 @@ class UniversalKriging3D(_Krige3DMixin, KrigeBase):
                         cols.append(np.asarray(func(xa, ya, za), dtype=float) * np.ones(xa.shape))
                 return np.ascontiguousarray(np.vstack(cols), dtype=np.float64)
 
-        kvalues, sigmasq = self._run_cuda(style, axes, flat_mask, drift_at=drift_at, dtype=dtype, n_gpus=n_gpus)
+        fields, one = self._check_values(values, dtype, None, n_gpus)
+        kvalues, sigmasq = self._run_cuda(style, axes, flat_mask, drift_at=drift_at, dtype=dtype, n_gpus=n_gpus,
+                                          **self._fields_kw(fields))
+        if one:
+            kvalues = kvalues[0]
         return self._shape_output(style, kvalues, sigmasq, sizes, flat_mask)
