@@ -350,6 +350,26 @@ int kb200_experimental_variogram(kb200_handle h, int dim, int64_t n,
  */
 int kb200_statistics(kb200_handle h, double* delta, double* sigma);
 
+/* Leave-one-out cross-validation of every station (DESIGN.md §5e). For station i, z and sigmasq are what the
+ * reference's execute('points') at station i returns for an object built from the other n - 1 stations with the
+ * same fixed variogram, anisotropy, coordinate type, exact_values and drift terms (the drift values at station i are
+ * its own row of the drift data). Host arrays: z as max(1, n_fields) blocks of n in station order (field f at
+ * z + f * n), sigmasq as n values.
+ *
+ * kb200_loo runs after kb200_set_problem on THIS handle, from the inverse factor it holds (no new factorisation):
+ * one pass over W = L^-1 (or the diagonal of C^-1 on the indefinite fallback) plus O(n (K + 1) V) work. A problem set
+ * with dtype KB200_F32 or KB200_F64X* is evaluated from the same fp64 factor, i.e. in fp64.
+ * Errors: KB200_ESTATE without a factored problem or for a problem received through kb200_blob_commit;
+ * KB200_EUNSUPPORTED with the pseudo-inverse, or when a station has more than 32 other stations within eps under
+ * exact_values; KB200_ESINGULAR when leaving a station out leaves the drift terms undetermined (|P_ii| at or below
+ * 1e-10 of its terms; the message names the lowest such station).
+ *
+ * kb200_knn_loo runs after kb200_set_problem_knn: the moving window with k neighbours taken from the other n - 1
+ * stations (ties by (d^2, original index) as kb200_execute_knn_*). 2 <= k <= n - 1 and the shared-memory limit of
+ * kb200_execute_knn_* (KB200_EBADARG / KB200_EUNSUPPORTED); a singular local system is KB200_ESINGULAR. */
+int kb200_loo(kb200_handle h, double* z, double* sigmasq);
+int kb200_knn_loo(kb200_handle h, int k, double* z, double* sigmasq);
+
 /* Debug/verification taps (used by tests only): copy device intermediates to host.
  *  what = 1: Cholesky factor L of the shifted covariance matrix (n_pad x n_pad, row-major, lower triangle valid)
  *  what = 2: W = inv(L) (same layout)

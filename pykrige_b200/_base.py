@@ -575,6 +575,37 @@ class KrigeBase:
             zs.append(np.reshape(z, (chunk.shape[0], -1)))
         return self._scatter(plan, np.concatenate(zs), ss)
 
+    # ---- leave_one_out(): cross-validation of every station --------------------------------------------------
+    def _leave_one_out(self, n_closest_points, values, backend, what):
+        """(zvalues, sigmasq) of kriging every station from the other N - 1 with this object's fixed variogram
+        (DESIGN.md §5e): the global path from the factorisation the last float64 execute() left on the handle (or a
+        new one, which a later execute() reuses), the moving window with n_closest_points neighbours. values as in
+        execute(values=...): zvalues is (V, N) for a 2-D values, (N,) otherwise; sigmasq is (N,)."""
+        self._check_backend(backend, what)
+        n = int(np.size(self._data_arrays()[3]))
+        if n < 2:
+            raise ValueError("leave-one-out needs at least two data points, got %d" % n)
+        knn = n_closest_points is not None
+        if knn and not 2 <= n_closest_points <= n - 1:
+            raise ValueError("leave-one-out: n_closest_points must be in [2, N - 1] = [2, %d], got %r"
+                             % (n - 1, n_closest_points))
+        if not knn and bool(getattr(self, "pseudo_inv", False)):
+            raise NotImplementedError("leave_one_out() has no pseudo_inv=True form on the global path: the "
+                                      "leave-one-out identities need the inverse of the kriging matrix")
+        fields, one = self._check_values(values, "float64", n_closest_points, None)
+
+        def run(h):
+            return h.knn_loo(int(n_closest_points), n) if knn else h.loo(n)
+        if fields is None:
+            return run(self._ensure_problem("float64", knn))
+        zs = []
+        for c0 in range(0, fields.shape[0], _cabi.MAX_FIELDS):
+            chunk = fields[c0:c0 + _cabi.MAX_FIELDS]
+            z, ss = run(self._ensure_problem("float64", knn, fields=chunk))
+            zs.append(np.reshape(z, (chunk.shape[0], n)))
+        z = np.concatenate(zs)
+        return (z[0] if one else z), ss
+
     @staticmethod
     def _check_backend(backend, what):
         if backend != "cuda":

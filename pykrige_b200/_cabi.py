@@ -38,7 +38,7 @@ EXPORTS = [
     "kb200_set_problem_knn",
     "kb200_blob_bytes", "kb200_blob_ptr", "kb200_describe_problem", "kb200_blob_commit",
     "kb200_set_coordinates", "kb200_set_stream", "kb200_last_timings", "kb200_reset_counters", "kb200_debug_fetch",
-    "kb200_experimental_variogram", "kb200_statistics", "kb200_set_pseudo_inverse",
+    "kb200_experimental_variogram", "kb200_statistics", "kb200_loo", "kb200_knn_loo", "kb200_set_pseudo_inverse",
     "kb200_set_variogram_table", "kb200_set_device_drift", "kb200_set_values",
     "kb200_group_create", "kb200_group_destroy", "kb200_group_last_error", "kb200_group_size", "kb200_group_member",
     "kb200_group_set_problem", "kb200_group_set_problem_knn", "kb200_group_execute_points",
@@ -101,6 +101,8 @@ def load_library():
     lib.kb200_debug_fetch.restype = i64
     lib.kb200_experimental_variogram.argtypes = [h, i32, i64, dp, dp, dp, dp, i32, dp, dp, dp, dp]
     lib.kb200_statistics.argtypes = [h, dp, dp]
+    lib.kb200_loo.argtypes = [h, dp, dp]
+    lib.kb200_knn_loo.argtypes = [h, i32, dp, dp]
     lib.kb200_set_pseudo_inverse.argtypes = [h, i32]
     lib.kb200_set_variogram_table.argtypes = [h, i64, ctypes.c_double, dp]
     lib.kb200_set_device_drift.argtypes = [h, i32, dp, i64, i64, dp, dp, dp]
@@ -401,6 +403,21 @@ class Handle:
         sigma = np.zeros(int(n))
         self._check(self.lib.kb200_statistics(self._h, _ptr(delta), _ptr(sigma)))
         return delta, sigma
+
+    def loo(self, n):
+        """Leave-one-out of every station of the problem kb200_set_problem factored on this handle (kb200_loo):
+        (z, sigmasq), z as max(1, n_fields) blocks of the n stations."""
+        z = np.empty(max(1, self.n_fields) * int(n), dtype=np.float64)
+        ss = np.empty(int(n), dtype=np.float64)
+        self._check(self.lib.kb200_loo(self._h, _ptr(z), _ptr(ss)))
+        return z, ss
+
+    def knn_loo(self, k, n):
+        """Moving-window leave-one-out of every station with k neighbours from the other n - 1 (kb200_knn_loo)."""
+        z = np.empty(max(1, self.n_fields) * int(n), dtype=np.float64)
+        ss = np.empty(int(n), dtype=np.float64)
+        self._check(self.lib.kb200_knn_loo(self._h, int(k), _ptr(z), _ptr(ss)), knn=True)
+        return z, ss
 
     def debug_fetch(self, what, count):
         out = np.empty(int(count), dtype=np.float64)

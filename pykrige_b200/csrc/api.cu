@@ -10,6 +10,7 @@
 #include <cstdlib>
 #include <algorithm>
 #include <thread>
+#include <climits>
 #include "kernels.h"
 
 #define KB_VERSION 2000
@@ -52,6 +53,7 @@ struct kb200_ctx {
     // description
     bool described = false, ready = false, knn_ready = false;
     bool factor_live = false;  // L (wC) and the forward solves (wF) of the ready problem are still in the workspace
+    bool inv_live = false;     // W (wW) or G (wC), the dual block (wF) and the values (wRaw) of kb200_set_problem: LOO
     int slices = 0;           // int8-slice dtypes: number of slices (6 / 5 / 4), else 0
     int gform = 0;            // 1: general (indefinite) fallback, tiles hold the symmetric inverse
     int geo = 0;              // 1: coordinates_type='geographic' for the next problem description
@@ -94,6 +96,7 @@ struct kb200_ctx {
     // knn workspace
     DevBuf kSorted, kCells, kFields;
     DevBuf wVario;            // constructor-side helpers (experimental variogram, statistics)
+    DevBuf wLoo;              // leave-one-out workspace
     DevBuf wTab;              // KB200_VG_TABLE: (value, slope) pairs on the device
     std::vector<double> htab; // ... and on the host (value, slope interleaved), for the covariance shift
     double tab_dmax = 0.0; int tab_n = 0;
@@ -144,7 +147,7 @@ extern "C" void kb200_destroy(kb200_handle h) {
     cudaStreamSynchronize(h->stream);
     for (DevBuf* b : {&h->blob, &h->wC, &h->wW, &h->wT, &h->wF, &h->wRaw, &h->wFlag, &h->wPart, &h->wAux,
                       &h->wPts, &h->wOut, &h->wAxes, &h->wDrift, &h->wScratch, &h->wFstage, &h->kSorted, &h->kCells, &h->kFields, &h->wVario, &h->wTab,
-                      &h->wWells, &h->wExt}) b->release();
+                      &h->wLoo, &h->wWells, &h->wExt}) b->release();
     for (int i = 0; i < 2; ++i) {
         if (h->pin[i]) cudaFreeHost(h->pin[i]);
         if (h->evk[i]) cudaEventDestroy(h->evk[i]);
@@ -268,7 +271,7 @@ static int describe(kb200_ctx* h, bool knn_only, int dim, int dtype, int64_t n,
                     const double* center, const double* aniso, int model, const double* vparams, int n_vparams,
                     int exact_values, double eps, int n_rl, int n_hd, const double* drift_data) {
     if (!h) return KB200_EBADARG;
-    h->described = false; h->ready = false; h->knn_ready = false; h->factor_live = false;
+    h->described = false; h->ready = false; h->knn_ready = false; h->factor_live = false; h->inv_live = false;
     if (dim != 2 && dim != 3) return fail(h, KB200_EBADARG, "dim must be 2 or 3");
     if (h->geo && dim != 2) return fail(h, KB200_EBADARG, "geographic coordinates are two-dimensional (lon, lat)");
     if (h->geo && (n_rl || n_hd)) return fail(h, KB200_EUNSUPPORTED, "universal kriging has no geographic mode (uk.py:337)");
@@ -617,6 +620,7 @@ extern "C" int kb200_set_problem(kb200_handle h, int dim, int dtype, int64_t n,
     if (hflag != 0) return fail(h, KB200_ESINGULAR, "drift/unbiasedness block F^T C^-1 F is singular");
     h->ready = true;
     h->factor_live = !h->gform;
+    h->inv_live = h->gform != 2;
     return KB200_OK;
 }
 
@@ -738,7 +742,7 @@ static int run_solve(kb200_ctx* h, const Src& s, double* d_z, double* d_ss) {
     return KB200_OK;
 }
 
-static int run_knn(kb200_ctx* h, int k, const Src& s, double* d_z, double* d_ss, int chol);
+static int run_knn(kb200_ctx* h, int k, const Src& s, double* d_z, double* d_ss, int chol, int loo = 0);
 
 // Launch `total` points in chunks and bring (z, ss) to the caller's HOST buffers. Large outputs travel through two
 // pinned staging buffers on a second stream while the next chunk computes; the host drains a buffer into the
@@ -1032,7 +1036,7 @@ extern "C" int kb200_set_problem_knn(kb200_handle h, int dim, int64_t n,
 
 
 // ---- moving window: execute ---------------------------------------------------------------------------------
-static int run_knn(kb200_ctx* h, int k, const Src& s, double* d_z, double* d_ss, int chol) {
+static int run_knn(kb200_ctx* h, int k, const Src& s, double* d_z, double* d_ss, int chol, int loo) {
     cudaStream_t st = h->stream;
     KnnParams kp = h->kp;
     kp.vg = h->vg; kp.an = h->an; kp.k = k;
@@ -1049,7 +1053,7 @@ static int run_knn(kb200_ctx* h, int k, const Src& s, double* d_z, double* d_ss,
     ps.px = s.a; ps.py = s.b; ps.pz = s.c; ps.gx = s.a; ps.gy = s.b; ps.gz = s.c;
     ps.nx = s.nx; ps.ny = s.ny; ps.nz = s.nz; ps.first = s.first;
     kp.ps = ps; kp.m = s.count; kp.z_out = d_z; kp.ss_out = d_ss; kp.flag = h->wFlag.as<int>(); kp.zstride = h->zstride;
-    CU(h, kbk_knn_solve(kp, chol, st));
+    CU(h, kbk_knn_solve(kp, chol, st, loo));
     h->launches += 1; h->solve_launches += 1;
     return KB200_OK;
 }
@@ -1068,12 +1072,12 @@ static int check_knn(kb200_ctx* h, int k) {
 // definite (variogram not valid in this dimension) -> repeat with the pivoted-LU solver (dgesv semantics);
 // 1 = exactly singular local system -> ValueError('Singular matrix') (cok.pyx:176-179).
 template <class MakeSrc>
-static int knn_to_host(kb200_ctx* h, int k, int64_t total, double* z_out, double* ss_out, MakeSrc make_src) {
+static int knn_to_host(kb200_ctx* h, int k, int64_t total, double* z_out, double* ss_out, MakeSrc make_src, int loo = 0) {
     int* flag = h->wFlag.as<int>();
     for (int chol = 1; chol >= 0; --chol) {
         CU(h, cudaMemsetAsync(flag, 0, sizeof(int), h->stream));
         int rc = run_to_host(h, total, z_out, ss_out, [&](int64_t o, int64_t c, double* dz, double* dss) {
-            return run_knn(h, k, make_src(o, c), dz, dss, chol);
+            return run_knn(h, k, make_src(o, c), dz, dss, chol, loo);
         });
         if (rc) return rc;
         int hflag = 0;
@@ -1439,4 +1443,105 @@ extern "C" int64_t kb200_debug_fetch(kb200_handle h, int what, double* out, int6
     if ((int64_t)cnt > cap) return KB200_EBADARG;
     if (cudaMemcpy(out, src, cnt * 8, cudaMemcpyDeviceToHost) != cudaSuccess) return KB200_ECUDA;
     return (int64_t)cnt;
+}
+
+// ---- leave-one-out cross-validation of every station (DESIGN.md §5e) ---------------------------------------------
+// |P_ii| at or below this fraction of its two terms is the rounding noise of their difference: without station i the
+// drift block is singular (e.g. universal kriging with n - 1 < K + 1 stations, or the rest collinear for a linear drift)
+static const double KB_LOO_TOL = 1e-10;
+
+extern "C" int kb200_loo(kb200_handle h, double* z_out, double* ss_out) {
+    if (!h || !z_out || !ss_out) return KB200_EBADARG;
+    if (!h->ready) return fail(h, KB200_ESTATE, "no factored problem: call kb200_set_problem first");
+    if (h->gform == 2) return fail(h, KB200_EUNSUPPORTED, "leave-one-out needs the inverse of the kriging matrix; "
+                                   "the pseudo-inverse (pseudo_inv=True) does not give it");
+    if (!h->inv_live) return fail(h, KB200_ESTATE, "the factorisation is not on this handle "
+                                  "(problem received through kb200_blob_commit)");
+    cudaSetDevice(h->device);
+    cudaStream_t st = h->stream;
+    const int nn = h->n, np = h->n_pad, nv = h->nf ? h->nf : 1;
+    const int nch = (nn + LOO_RC - 1) / LOO_RC;
+    // doubles: part [nch][n] | pii [n] | alpha [nv][n] | z [nv][n] | ss [n], then ints: cnt [n] | off [n + 1] | st [n] | bad
+    const size_t nd = ((size_t)nch + 2 + 2 * (size_t)nv) * nn, ni = 3 * (size_t)nn + 2;
+    CU(h, h->wLoo.reserve(nd * sizeof(double) + ni * sizeof(int)));
+    double* part = h->wLoo.as<double>();
+    double* pii = part + (size_t)nch * nn;
+    double* alpha = pii + nn;
+    double* dz = alpha + (size_t)nv * nn;
+    double* dss = dz + (size_t)nv * nn;
+    int* cnt = reinterpret_cast<int*>(h->wLoo.as<double>() + nd);
+    int* off = cnt + nn;
+    int* slist = off + nn + 1;
+    int* bad = slist + nn;
+    char* blob = h->blob.as<char>();
+    const double* ax = reinterpret_cast<double*>(blob + h->off_ax);
+    const double* ay = reinterpret_cast<double*>(blob + h->off_ay);
+    const double* az = reinterpret_cast<double*>(blob + h->off_az);
+    const double* raw = h->wRaw.as<double>();
+    int launches = 0;
+
+    // exact_values: stations within eps of each other (counts, then the lists at host-scanned offsets)
+    std::vector<int> hcnt, hoff, hst;
+    int* pj = nullptr; double* pd = nullptr;
+    if (h->vg.exact) {
+        CU(h, kbk_loo_pairs(h->dim, nn, ax, ay, az, h->vg.eps, cnt, nullptr, nullptr, nullptr, st)); ++launches;
+        hcnt.resize(nn);
+        CU(h, cudaMemcpyAsync(hcnt.data(), cnt, (size_t)nn * sizeof(int), cudaMemcpyDeviceToHost, st));
+        CU(h, cudaStreamSynchronize(st));
+        hoff.assign(nn + 1, 0);
+        for (int i = 0; i < nn; ++i) {
+            if (hcnt[i] > LOO_MAXDUP)
+                return fail(h, KB200_EUNSUPPORTED, "leave-one-out: station " + std::to_string(i) + " has " +
+                            std::to_string(hcnt[i]) + " other stations within eps (at most " + std::to_string(LOO_MAXDUP) + ")");
+            hoff[i + 1] = hoff[i] + hcnt[i];
+            if (hcnt[i]) hst.push_back(i);
+        }
+        if (hoff[nn] > 0) {
+            const size_t tot = (size_t)hoff[nn];
+            CU(h, h->wVario.reserve(tot * (sizeof(double) + sizeof(int))));
+            pd = h->wVario.as<double>();
+            pj = reinterpret_cast<int*>(pd + tot);
+            CU(h, cudaMemcpyAsync(off, hoff.data(), (size_t)(nn + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
+            CU(h, cudaMemcpyAsync(slist, hst.data(), hst.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+            CU(h, kbk_loo_pairs(h->dim, nn, ax, ay, az, h->vg.eps, cnt, off, pj, pd, st)); ++launches;
+        }
+    }
+
+    LooParams p{};
+    p.n = nn; p.n_pad = np; p.ld = h->ld; p.K1 = h->K1; p.nv = nv; p.gform = h->gform; p.nchunks = nch;
+    p.tol = KB_LOO_TOL; p.vg = h->vg;
+    p.W = h->wW.as<double>(); p.G = h->wC.as<double>(); p.part = part;
+    p.Uz = h->wF.as<double>() + (size_t)2 * h->aux_cols * np;
+    p.consts = reinterpret_cast<const double*>(blob + h->off_consts);
+    p.Z = h->nf ? raw + (size_t)(4 + h->n_hd) * nn : raw + 3 * (size_t)nn;      // wRaw: x | y | z | v | drift | fields
+    p.pii = pii; p.alpha = alpha; p.z_out = dz; p.ss_out = dss; p.bad = bad;
+    const int big = INT_MAX;
+    CU(h, cudaMemcpyAsync(bad, &big, sizeof(int), cudaMemcpyHostToDevice, st));
+    CU(h, cudaEventRecord(h->ev[7], st));
+    if (h->gform == 0) { CU(h, kbk_loo_colsq(p.W, p.ld, nn, part, st)); ++launches; }
+    CU(h, kbk_loo_finalize(p, st)); ++launches;
+    if (!hst.empty()) { CU(h, kbk_loo_dup(p, (int)hst.size(), slist, off, pj, pd, st)); ++launches; }
+    CU(h, cudaEventRecord(h->ev[8], st));
+    int hbad = big;
+    CU(h, cudaMemcpyAsync(&hbad, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaMemcpyAsync(z_out, dz, (size_t)nv * nn * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaMemcpyAsync(ss_out, dss, (size_t)nn * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    h->tm[4] += ev_ms(h->ev[7], h->ev[8]);
+    h->launches += launches; h->solve_launches += launches;
+    if (hbad != big)
+        return fail(h, KB200_ESINGULAR, "leave-one-out: without station " + std::to_string(hbad) +
+                    " the drift terms are not determined (singular drift block)");
+    return KB200_OK;
+}
+
+extern "C" int kb200_knn_loo(kb200_handle h, int k, double* z_out, double* ss_out) {
+    int rc = check_knn(h, k); if (rc) return rc;
+    if (k > h->n - 1) return fail(h, KB200_EBADARG, "leave-one-out: n_closest_points must be at most n - 1");
+    if (!z_out || !ss_out) return fail(h, KB200_EBADARG, "null pointer");
+    const int nn = h->n;
+    const double* raw = h->wRaw.as<double>();      // the stations' raw coordinates are the query points
+    return knn_to_host(h, k, nn, z_out, ss_out, [&](int64_t o, int64_t c) {
+        return Src{false, 0, 0, 0, raw, raw + nn, raw + 2 * (size_t)nn, o, c, nullptr, 0, 0};
+    }, 1);
 }

@@ -251,7 +251,9 @@ struct KnnParams {
 cudaError_t kbk_knn_build(int dim, int n, const double* ax, const double* ay, const double* az, const double* values,
                           KnnParams& kp, double* sx, double* sy, double* sz, double* sv, int* sorig,
                           int* cell_of, int* cell_start, int* cursor, int ncells, cudaStream_t st, int* launches);
-cudaError_t kbk_knn_solve(const KnnParams& p, int chol, cudaStream_t st);
+// loo = 1: leave-one-out of every station, query p = station ps.first + p (ps = the raw station coordinates), and the
+// candidate with that original index is never counted
+cudaError_t kbk_knn_solve(const KnnParams& p, int chol, cudaStream_t st, int loo = 0);
 size_t      kbk_knn_smem_per_warp(int k, int chol, int hasz, int nv);
 // dst[v * n + s] = src[v * n + sorig[s]] for v < nv: value fields in the cell-sorted order of the moving window
 cudaError_t kbk_knn_sort_fields(int n, int nv, const int* sorig, const double* src, double* dst, cudaStream_t st);
@@ -269,6 +271,31 @@ cudaError_t kbk_ev_bin(int dim, int n, const double* x, const double* y, const d
 cudaError_t kbk_statistics(int dim, int n, const double* ax, const double* ay, const double* az,
                            const double* L, int ld, const double* u, const double* zeta, int* dup,
                            double* delta, double* sigma, cudaStream_t st);
+
+// loo.cu: leave-one-out cross-validation of every station from the held factorisation (DESIGN.md §5e)
+#define LOO_RC 256          // rows per chunk of the column sums of squares of W
+#define LOO_MAXDUP 32       // stations within eps of one station that the exact-hit correction handles
+struct LooParams {
+    int n, n_pad, ld, K1, nv, gform, nchunks;
+    double tol;                // |P_ii| <= tol * max(|diag term|, |u_i^T S^-1 u_i|): drift not determined without i
+    VgParams vg;
+    const double* W;           // gform 0: W = L^-1 (lower triangle, row-major, ld)
+    const double* G;           // gform 1: G = C^-1 (full, row-major, ld)
+    const double* part;        // gform 0: [nchunks][n] chunk sums of squares of W's columns
+    const double* Uz;          // [K1 + nv][n_pad]: U = C^-1 F (rescaled drift + ones), then zeta_v = C^-1 Z_v
+    const double* consts;      // S^-1 (K1 x K1), then phi_v (K1 each)
+    const double* Z;           // [nv][n] station values
+    double* pii; double* alpha;   // [n], [nv][n]: kept for the exact-hit correction
+    double* z_out; double* ss_out;   // [nv][n], [n]
+    int* bad;                  // lowest station whose P_ii is at rounding level (INT_MAX: none)
+};
+cudaError_t kbk_loo_colsq(const double* W, int ld, int n, double* part, cudaStream_t st);
+cudaError_t kbk_loo_finalize(const LooParams& p, cudaStream_t st);
+// off == NULL: cnt[i] = |D(i)|; else station i's near stations j (ascending) and distances at pj/pd + off[i]
+cudaError_t kbk_loo_pairs(int dim, int n, const double* ax, const double* ay, const double* az, double eps, int* cnt,
+                          const int* off, int* pj, double* pd, cudaStream_t st);
+cudaError_t kbk_loo_dup(const LooParams& p, int nst, const int* st_list, const int* off, const int* pj, const double* pd,
+                        cudaStream_t st);
 
 // pinv.cu: pseudo_inv=True (one-sided Jacobi SVD of the bordered kriging matrix)
 cudaError_t kbk_build_fz(int n, int n_pad, int n_rl, int n_hd, const double* ax, const double* ay, const double* az,

@@ -123,7 +123,10 @@ __device__ __forceinline__ void warp_bitonic(double* d2, int* id, const int* __r
 //               A non-positive pivot (variogram not valid in this dimension) sets *flag = 2 and the host
 //               re-runs the launch with CHOL = false.
 // CHOL = false: LU with partial pivoting on the full k x k block (dgesv semantics, cok.pyx:165-174).
-template <int DIM, int MODEL, bool CHOL>
+// LOO = true : leave-one-out of station q = ps.first + p (ps holds the raw station coordinates): the candidate with
+//              original index q is never counted. It lands at d^2 == 0 exactly (data and query go through the same
+//              adjust sequence), so only there is its index looked up.
+template <int DIM, int MODEL, bool CHOL, bool LOO = false>
 __global__ void __launch_bounds__(320) knn_solve_kernel(const __grid_constant__ KnnParams P, int warps_per_cta,
                                                          int per_warp_doubles) {
     extern __shared__ __align__(16) double ksm[];
@@ -201,7 +204,7 @@ __global__ void __launch_bounds__(320) knn_solve_kernel(const __grid_constant__ 
             const int total = __shfl_sync(0xffffffffu, incl, 31);
             for (int f0 = 0; f0 < total; f0 += 32) {
                 const int f = f0 + lane;
-                const bool ok = f < total;
+                bool ok = f < total;
                 int j = 0;
 #pragma unroll
                 for (int st = 16; st > 0; st >>= 1) {
@@ -218,6 +221,7 @@ __global__ void __launch_bounds__(320) knn_solve_kernel(const __grid_constant__ 
                     double dx = P.ax[i] - qx, dy = P.ay[i] - qy;
                     d2 = dx * dx + dy * dy;
                     if (KB_HASZ(DIM)) { double dz = P.az[i] - qz; d2 += dz * dz; }
+                    if (LOO && d2 == 0.0 && P.sorig[i] == P.ps.first + p) ok = false;
                 }
                 unsigned msk = __ballot_sync(0xffffffffu, ok);
                 int pos = cnt + __popc(msk & ((1u << lane) - 1u));
@@ -690,7 +694,7 @@ cudaError_t kbk_knn_sort_fields(int n, int nv, const int* sorig, const double* s
     return cudaGetLastError();
 }
 
-template <int DIM, bool CHOL>
+template <int DIM, bool CHOL, bool LOO>
 static cudaError_t knn_launch_dim(const KnnParams& p, cudaStream_t st) {
     size_t per = kbk_knn_smem_per_warp(p.k, CHOL ? 1 : 0, KB_HASZ(DIM) ? 1 : 0, p.nv);
     int wpc = (int)std::min<size_t>(10, (size_t)(226 * 1024) / per);   // as many points in flight per SM as fit (<= 320 threads; 227 KB minus the static 1 KB)
@@ -700,9 +704,9 @@ static cudaError_t knn_launch_dim(const KnnParams& p, cudaStream_t st) {
     int per_d = (int)(per / sizeof(double));
     switch (p.vg.model) {
 #define KB_CASE(M) case M: { \
-        cudaError_t e = cudaFuncSetAttribute(knn_solve_kernel<DIM, M, CHOL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+        cudaError_t e = cudaFuncSetAttribute(knn_solve_kernel<DIM, M, CHOL, LOO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
         if (e != cudaSuccess) return e; \
-        knn_solve_kernel<DIM, M, CHOL><<<grid, wpc * 32, smem, st>>>(p, wpc, per_d); } break;
+        knn_solve_kernel<DIM, M, CHOL, LOO><<<grid, wpc * 32, smem, st>>>(p, wpc, per_d); } break;
         KB_CASE(KB200_VG_LINEAR) KB_CASE(KB200_VG_POWER) KB_CASE(KB200_VG_GAUSSIAN)
         KB_CASE(KB200_VG_EXPONENTIAL) KB_CASE(KB200_VG_SPHERICAL) KB_CASE(KB200_VG_HOLE_EFFECT) KB_CASE(KB200_VG_TABLE)
 #undef KB_CASE
@@ -711,10 +715,15 @@ static cudaError_t knn_launch_dim(const KnnParams& p, cudaStream_t st) {
     return cudaGetLastError();
 }
 
-cudaError_t kbk_knn_solve(const KnnParams& p, int chol, cudaStream_t st) {
+template <bool LOO>
+static cudaError_t knn_solve_loo(const KnnParams& p, int chol, cudaStream_t st) {
     if (chol && p.k <= 128)
-        return p.dim == 2 ? knn_launch_dim<2, true>(p, st) : (p.dim == 3 ? knn_launch_dim<3, true>(p, st) : knn_launch_dim<KB_GEO, true>(p, st));
-    return p.dim == 2 ? knn_launch_dim<2, false>(p, st) : (p.dim == 3 ? knn_launch_dim<3, false>(p, st) : knn_launch_dim<KB_GEO, false>(p, st));
+        return p.dim == 2 ? knn_launch_dim<2, true, LOO>(p, st) : (p.dim == 3 ? knn_launch_dim<3, true, LOO>(p, st) : knn_launch_dim<KB_GEO, true, LOO>(p, st));
+    return p.dim == 2 ? knn_launch_dim<2, false, LOO>(p, st) : (p.dim == 3 ? knn_launch_dim<3, false, LOO>(p, st) : knn_launch_dim<KB_GEO, false, LOO>(p, st));
+}
+
+cudaError_t kbk_knn_solve(const KnnParams& p, int chol, cudaStream_t st, int loo) {
+    return loo ? knn_solve_loo<true>(p, chol, st) : knn_solve_loo<false>(p, chol, st);
 }
 
 cudaError_t kbk_knn_build(int dim, int n, const double* ax, const double* ay, const double* az, const double* values,

@@ -56,3 +56,17 @@ class OrdinaryKriging(Krige2DMixin, KrigeBase):
         if one:
             zvalues = zvalues[0]
         return self._shape_output(style, zvalues, sigmasq, sizes, flat_mask)
+
+    def leave_one_out(self, n_closest_points=None, values=None, backend="cuda"):
+        """Leave-one-out cross-validation: every station kriged from the other N - 1 stations with this object's fixed
+        variogram, anisotropy, coordinate type and ``exact_values`` (the variogram is not refitted per fold). Returns
+        ``(zvalues, sigmasq)`` in station order: ``zvalues`` (N,), or (V, N) for a 2-D ``values``; ``sigmasq`` (N,).
+        The residuals are ``values - zvalues`` and the standardised residuals divide them by ``sqrt(sigmasq)``.
+
+        Without ``n_closest_points`` the global path reads the factorisation the last float64 execute() left on the
+        device (or makes one, which a later execute() reuses): O(N^2) on top of it, not N factorisations.
+        ``n_closest_points = k`` (2 <= k <= N - 1) runs the moving window with k neighbours from the other stations.
+        ``values`` (shape (N,) or (N, V)) as in execute(values=...). ``pseudo_inv=True`` is refused on the global path
+        (NotImplementedError) and ignored by the moving window, as in execute().
+        """
+        return self._leave_one_out(n_closest_points, values, backend, "2D ordinary kriging")

@@ -117,3 +117,16 @@ class UniversalKriging3D(_Krige3DMixin, KrigeBase):
         if one:
             kvalues = kvalues[0]
         return self._shape_output(style, kvalues, sigmasq, sizes, flat_mask)
+
+    def leave_one_out(self, values=None, backend="cuda"):
+        """Leave-one-out cross-validation: every station kriged from the other N - 1 stations with this object's fixed
+        variogram, anisotropy, ``exact_values`` and drift terms (the drift values at a held-out station are its own row
+        of the drift data; the variogram is not refitted per fold). Returns ``(zvalues, sigmasq)`` in station order:
+        ``zvalues`` (N,), or (V, N) for a 2-D ``values``; ``sigmasq`` (N,).
+
+        Reads the factorisation the last float64 execute() left on the device (or makes one, which a later execute()
+        reuses): O(N^2) on top of it, not N factorisations. ``values`` (shape (N,) or (N, V)) as in
+        execute(values=...). Raises ``numpy.linalg.LinAlgError`` naming the station when leaving it out leaves the
+        drift terms undetermined, and NotImplementedError with ``pseudo_inv=True``.
+        """
+        return self._leave_one_out(None, values, backend, "3D Universal kriging")
