@@ -20,15 +20,32 @@ static const int64_t KB_STAGE_PTS = 1 << 20;   // prediction points per staged o
 static const int64_t KB_STAGE_MIN = 1 << 18;   // below this the outputs go straight to the caller's buffers
 #define KB_TN_FIELDS 32   // widest point tile of the value-fields solve kernels (solve.cu: no spills up to 32 points)
 
+// Prediction points on the device: [first, first + count) of the explicit points or of the flattened grid
 struct Src {
     bool grid; int64_t nx, ny, nz;
     const double *a, *b, *c;      // points (px,py,pz) or axes (gx,gy,gz), device pointers
     int64_t first, count;
     const double* d_drift; int64_t drift_stride, drift_first;
+
+    Src sub(int64_t o, int64_t m) const {        // points [o, o + m) of this source
+        Src s = *this; s.first += o; s.count = m; s.drift_first += o; return s;
+    }
+    PointSource point_source() const {
+        PointSource ps{};
+        ps.grid = grid ? 1 : 0;
+        ps.px = a; ps.py = b; ps.pz = c; ps.gx = a; ps.gy = b; ps.gz = c;
+        ps.nx = nx; ps.ny = ny; ps.nz = nz; ps.first = first;
+        return ps;
+    }
 };
 
-// general (indefinite) path: blocked Gauss-Jordan unless KB200_GJ=scalar
-#define KB_GJ_DEFAULT_BLOCKED 1
+// tm[] slots, in the order of kb200_last_timings (krige_b200.h) and _cabi.TIMING_KEYS
+enum Tm { TM_ASSEMBLE, TM_CHOLESKY, TM_TRTRI, TM_PACK_DUAL, TM_SOLVE, TM_FINALIZE, TM_H2D, TM_D2H, TM_KNN_SEARCH,
+          TM_KNN_SOLVE, TM_SOLVE_LAUNCHES, TM_LAUNCHES, TM_COUNT };
+// ev[] slots: the phases of kb200_set_problem (kb200_set_problem_knn: upload, then the cell grid build), the window
+// of an execute call's solve launches (run_to_host records it for its callers) and its host <-> device copies
+enum Ev { EV_UPLOAD, EV_ADJUSTED, EV_ASM, EV_KNN_BUILT = EV_ASM, EV_FACTOR, EV_INVERT, EV_DUAL, EV_PACKED,
+          EV_RUN, EV_RUN_END, EV_H2D, EV_H2D_END, EV_D2H_END, EV_COUNT };
 
 struct DevBuf {
     void* p = nullptr; size_t cap = 0;
@@ -52,8 +69,9 @@ struct kb200_ctx {
 
     // description
     bool described = false, ready = false, knn_ready = false;
-    bool factor_live = false;  // L (wC) and the forward solves (wF) of the ready problem are still in the workspace
-    bool inv_live = false;     // W (wW) or G (wC), the dual block (wF) and the values (wRaw) of kb200_set_problem: LOO
+    // kb200_set_problem factored the problem on this handle (not kb200_blob_commit): its factor or inverse (wC, wW),
+    // dual blocks (wF) and data (wRaw) are in the workspace
+    bool local_factor = false;
     int slices = 0;           // int8-slice dtypes: number of slices (6 / 5 / 4), else 0
     int gform = 0;            // 1: general (indefinite) fallback, tiles hold the symmetric inverse
     int geo = 0;              // 1: coordinates_type='geographic' for the next problem description
@@ -73,14 +91,13 @@ struct kb200_ctx {
     int64_t zstride = 0;       // z_out block stride of the fields in the running execute call
     int pin_blocks = 0;        // capacity of each pinned staging buffer, in blocks of KB_STAGE_PTS doubles
 
-    // blob (one allocation): header | consts | ax | ay | az | tiles
-    DevBuf blob;
+    DevBuf blob;              // the factor blob (BlobView)
     size_t off_consts = 0, off_ax = 0, off_ay = 0, off_az = 0, off_tiles = 0, off_rowscale = 0, blob_bytes = 0;
 
     // factor workspace
     DevBuf wC, wW, wT, wF, wRaw, wFlag;
     // execute workspace
-    DevBuf wPart, wAux, wPts, wOut, wAxes, wDrift, wScratch, wFstage;
+    DevBuf wPts, wOut, wDrift, wScratch, wFstage;
     int num_sms = 132;
     // device-evaluated drift terms (kb200_set_device_drift): configuration + the count used by the described problem
     DeviceDrift dd{};
@@ -103,8 +120,8 @@ struct kb200_ctx {
     KnnParams kp{};
     int k_ncells = 0;
 
-    cudaEvent_t ev[16] = {};
-    double tm[12] = {};
+    cudaEvent_t ev[EV_COUNT] = {};
+    double tm[TM_COUNT] = {};
     long long launches = 0, solve_launches = 0;
 };
 
@@ -117,6 +134,52 @@ static int fail(kb200_ctx* h, int code, const std::string& msg) {
                 std::string(#expr) + ": " + cudaGetErrorString(_e)); } } while (0)
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+// Every setter changes what the next description means: the described (and any factored) problem is gone
+static void drop_problem(kb200_ctx* h) {
+    h->described = false; h->ready = false; h->knn_ready = false; h->local_factor = false;
+}
+
+// The factor blob, one allocation that multigpu.py ships between processes built from the same commit:
+// header | consts (S^-1 | phi_v) | ax | ay | az (adjusted data coordinates) | tiles | rowscale (int8-slice dtypes)
+struct BlobView { double *hdr, *consts, *ax, *ay, *az; char* tiles; double* rowscale; };
+static BlobView blob_view(const kb200_ctx* h) {
+    char* p = h->blob.as<char>();
+    auto at = [p](size_t off) { return reinterpret_cast<double*>(p + off); };
+    return {at(0), at(h->off_consts), at(h->off_ax), at(h->off_ay), at(h->off_az), p + h->off_tiles, at(h->off_rowscale)};
+}
+
+// blob header slots (doubles): magic, c0, drift shift and scale per column, gform
+enum HdrSlot { HDR_MAGIC = 0, HDR_C0 = 1, HDR_SHIFT = 2, HDR_SCALE = HDR_SHIFT + KB200_MAX_DRIFT + 1,
+               HDR_GFORM = HDR_SCALE + KB200_MAX_DRIFT + 1, HDR_DOUBLES = 64 };
+static_assert(HDR_GFORM == 34 && HDR_GFORM < HDR_DOUBLES, "blob header layout");
+static const double KB_MAGIC = 20260922.0;
+
+static void write_header(const kb200_ctx* h, double* hdr) {
+    std::fill(hdr, hdr + HDR_DOUBLES, 0.0);
+    hdr[HDR_MAGIC] = KB_MAGIC; hdr[HDR_C0] = h->vg.c0; hdr[HDR_GFORM] = (double)h->gform;
+    for (int c = 0; c <= KB200_MAX_DRIFT; ++c) { hdr[HDR_SHIFT + c] = h->ds.shift[c]; hdr[HDR_SCALE + c] = h->ds.scale[c]; }
+}
+
+static bool read_header(kb200_ctx* h, const double* hdr) {
+    if (hdr[HDR_MAGIC] != KB_MAGIC) return false;
+    h->vg.c0 = hdr[HDR_C0];
+    h->gform = (int)hdr[HDR_GFORM];
+    for (int c = 0; c <= KB200_MAX_DRIFT; ++c) { h->ds.shift[c] = hdr[HDR_SHIFT + c]; h->ds.scale[c] = hdr[HDR_SCALE + c]; }
+    return true;
+}
+
+// wRaw: the raw data columns x | y | z | values | n_hd drift columns | nf value fields, n doubles each
+enum RawCol { RAW_X, RAW_Y, RAW_Z, RAW_V, RAW_DRIFT };
+static double* raw_col(const kb200_ctx* h, int c) { return h->wRaw.as<double>() + (size_t)c * h->n; }
+// the values the problem kriges: its own, or the nf value fields of kb200_set_values
+static double* kriged_values(const kb200_ctx* h) { return raw_col(h, h->nf ? RAW_DRIFT + h->n_hd : RAW_V); }
+
+// wF: Fz | Hz | Uz, aux_cols columns of n_pad each
+enum AuxBlock { AUX_F, AUX_H, AUX_U };
+static double* aux_block(const kb200_ctx* h, int i) {
+    return h->wF.as<double>() + (size_t)i * h->aux_cols * h->n_pad;
+}
 
 extern "C" int kb200_version(void) { return KB_VERSION; }
 
@@ -145,8 +208,8 @@ extern "C" void kb200_destroy(kb200_handle h) {
     if (!h) return;
     cudaSetDevice(h->device);
     cudaStreamSynchronize(h->stream);
-    for (DevBuf* b : {&h->blob, &h->wC, &h->wW, &h->wT, &h->wF, &h->wRaw, &h->wFlag, &h->wPart, &h->wAux,
-                      &h->wPts, &h->wOut, &h->wAxes, &h->wDrift, &h->wScratch, &h->wFstage, &h->kSorted, &h->kCells, &h->kFields, &h->wVario, &h->wTab,
+    for (DevBuf* b : {&h->blob, &h->wC, &h->wW, &h->wT, &h->wF, &h->wRaw, &h->wFlag,
+                      &h->wPts, &h->wOut, &h->wDrift, &h->wScratch, &h->wFstage, &h->kSorted, &h->kCells, &h->kFields, &h->wVario, &h->wTab,
                       &h->wLoo, &h->wWells, &h->wExt}) b->release();
     for (int i = 0; i < 2; ++i) {
         if (h->pin[i]) cudaFreeHost(h->pin[i]);
@@ -176,20 +239,20 @@ extern "C" int kb200_set_coordinates(kb200_handle h, int coordinates_type) {
     if (coordinates_type != KB200_EUCLIDEAN && coordinates_type != KB200_GEOGRAPHIC)
         return fail(h, KB200_EBADARG, "coordinates_type must be KB200_EUCLIDEAN or KB200_GEOGRAPHIC");
     h->geo = coordinates_type == KB200_GEOGRAPHIC ? 1 : 0;
-    h->described = false; h->ready = false; h->knn_ready = false; h->factor_live = false;
+    drop_problem(h);
     return KB200_OK;
 }
 
 extern "C" int kb200_set_pseudo_inverse(kb200_handle h, int enable) {
     if (!h) return KB200_EBADARG;
     h->pinv = enable ? 1 : 0;
-    h->described = false; h->ready = false; h->knn_ready = false; h->factor_live = false;
+    drop_problem(h);
     return KB200_OK;
 }
 
 extern "C" int kb200_set_values(kb200_handle h, int n_fields, int64_t n, const double* values) {
     if (!h) return KB200_EBADARG;
-    h->described = false; h->ready = false; h->knn_ready = false; h->factor_live = false;
+    drop_problem(h);
     h->nf = 0; h->nf_n = 0; h->hfields.clear();
     if (n_fields == 0) return KB200_OK;
     if (n_fields < 0 || n_fields > KB200_MAX_FIELDS)
@@ -213,9 +276,9 @@ extern "C" void kb200_reset_counters(kb200_handle h) {
 
 extern "C" int kb200_last_timings(kb200_handle h, double* ms, int n) {
     if (!h || !ms) return KB200_EBADARG;
-    h->tm[10] = (double)h->solve_launches;
-    h->tm[11] = (double)h->launches;
-    int m = std::min(n, 12);
+    h->tm[TM_SOLVE_LAUNCHES] = (double)h->solve_launches;
+    h->tm[TM_LAUNCHES] = (double)h->launches;
+    int m = std::min(n, (int)TM_COUNT);
     for (int i = 0; i < m; ++i) ms[i] = h->tm[i];
     return m;
 }
@@ -246,7 +309,7 @@ extern "C" int kb200_set_variogram_table(kb200_handle h, int64_t n_nodes, double
     const int n = (int)n_nodes;
     for (int i = 0; i < n; ++i)
         if (!std::isfinite(gamma_nodes[i])) return fail(h, KB200_EBADARG, "variogram table: the callable must be finite on [0, dmax] (node " + std::to_string(i) + ")");
-    h->described = false; h->ready = false; h->knn_ready = false; h->factor_live = false;
+    drop_problem(h);
     // slopes per unit node index: centred differences, second-order one-sided at the two ends
     h->htab.resize(2 * (size_t)n);
     for (int i = 0; i < n; ++i) {
@@ -271,7 +334,7 @@ static int describe(kb200_ctx* h, bool knn_only, int dim, int dtype, int64_t n,
                     const double* center, const double* aniso, int model, const double* vparams, int n_vparams,
                     int exact_values, double eps, int n_rl, int n_hd, const double* drift_data) {
     if (!h) return KB200_EBADARG;
-    h->described = false; h->ready = false; h->knn_ready = false; h->factor_live = false; h->inv_live = false;
+    drop_problem(h);
     if (dim != 2 && dim != 3) return fail(h, KB200_EBADARG, "dim must be 2 or 3");
     if (h->geo && dim != 2) return fail(h, KB200_EBADARG, "geographic coordinates are two-dimensional (lon, lat)");
     if (h->geo && (n_rl || n_hd)) return fail(h, KB200_EUNSUPPORTED, "universal kriging has no geographic mode (uk.py:337)");
@@ -303,7 +366,6 @@ static int describe(kb200_ctx* h, bool knn_only, int dim, int dtype, int64_t n,
     }
     h->slices = dtype == KB200_F64X ? 6 : dtype == KB200_F64X5 ? 5 : dtype == KB200_F64X4 ? 4 : 0;
 
-    const int user_dim = dim;
     h->dim = h->geo ? KB_GEO : dim; h->dtype = dtype; h->n = (int)n; h->n_rl = n_rl; h->n_hd = n_hd;
     // dual rows: K + 1 drift/unbiasedness rows and one zeta row per value field (n + na <= n + 80 stays within
     // KB_MAXRB row blocks for every n the check above admits)
@@ -328,7 +390,6 @@ static int describe(kb200_ctx* h, bool knn_only, int dim, int dtype, int64_t n,
 
     // adjusted bounding box on the host (drift rescale + c0 for unbounded models)
     double lo[3] = {1e300, 1e300, 1e300}, hi[3] = {-1e300, -1e300, -1e300};
-    (void)user_dim;
     const int sdim = h->geo ? 3 : dim;            // spatial dimensions of the device coordinates
     for (int64_t i = 0; i < n; ++i) {
         if (h->geo) {
@@ -396,7 +457,7 @@ static int describe(kb200_ctx* h, bool knn_only, int dim, int dtype, int64_t n,
     }
     size_t esz = 8;   // fp64 value, or TF32 hi + lo pair: both 8 bytes per element
     size_t o = 0;
-    o += align_up(64 * sizeof(double), 256);
+    o += align_up(HDR_DOUBLES * sizeof(double), 256);
     h->off_consts = o; o += align_up((size_t)std::max(512, h->K1 * h->na) * sizeof(double), 256);   // S^-1 | phi_v
     h->off_ax = o; o += align_up((size_t)h->n_pad * 8, 256);
     h->off_ay = o; o += align_up((size_t)h->n_pad * 8, 256);
@@ -429,24 +490,132 @@ extern "C" int kb200_describe_problem(kb200_handle h, int dim, int dtype, int64_
 extern "C" int64_t kb200_blob_bytes(kb200_handle h) { return (h && h->described) ? (int64_t)h->blob_bytes : 0; }
 extern "C" void* kb200_blob_ptr(kb200_handle h) { return (h && h->described) ? h->blob.p : nullptr; }
 
-// header layout (doubles): [0] magic, [1] c0, [2..18) shift, [18..34) scale
-static const double KB_MAGIC = 20260922.0;
-
 extern "C" int kb200_blob_commit(kb200_handle h) {
     if (!h || !h->described) return fail(h, KB200_ESTATE, "describe the problem first");
     cudaSetDevice(h->device);
-    double hdr[64];
+    double hdr[HDR_DOUBLES];
     CU(h, cudaMemcpyAsync(hdr, h->blob.p, sizeof(hdr), cudaMemcpyDeviceToHost, h->stream));
     CU(h, cudaStreamSynchronize(h->stream));
-    if (hdr[0] != KB_MAGIC) return fail(h, KB200_ESTATE, "blob does not hold a factored problem");
-    h->vg.c0 = hdr[1];
-    h->gform = (int)hdr[34];
-    for (int c = 0; c <= KB200_MAX_DRIFT; ++c) { h->ds.shift[c] = hdr[2 + c]; h->ds.scale[c] = hdr[18 + c]; }
+    if (!read_header(h, hdr)) return fail(h, KB200_ESTATE, "blob does not hold a factored problem");
     h->ready = true;
     return KB200_OK;
 }
 
 static float ev_ms(cudaEvent_t a, cudaEvent_t b) { float t = 0.f; cudaEventElapsedTime(&t, a, b); return t; }
+
+// The described data to wRaw (with `fields`, the value fields too) and its adjusted coordinates to the blob axes,
+// zero beyond n. Timed as h2d: EV_UPLOAD .. EV_ADJUSTED.
+static int upload_data(kb200_ctx* h, bool fields, int* launches) {
+    cudaStream_t st = h->stream;
+    const size_t col = (size_t)h->n * sizeof(double);
+    CU(h, h->wRaw.reserve((4 + h->n_hd + (fields ? h->nf : 0)) * col));
+    const BlobView b = blob_view(h);
+    CU(h, cudaEventRecord(h->ev[EV_UPLOAD], st));
+    CU(h, cudaMemcpyAsync(raw_col(h, RAW_X), h->hx.data(), col, cudaMemcpyHostToDevice, st));
+    CU(h, cudaMemcpyAsync(raw_col(h, RAW_Y), h->hy.data(), col, cudaMemcpyHostToDevice, st));
+    CU(h, cudaMemcpyAsync(raw_col(h, RAW_Z), h->hz.data(), col, cudaMemcpyHostToDevice, st));
+    CU(h, cudaMemcpyAsync(raw_col(h, RAW_V), h->hval.data(), col, cudaMemcpyHostToDevice, st));
+    if (h->n_hd) CU(h, cudaMemcpyAsync(raw_col(h, RAW_DRIFT), h->hdrift.data(), h->n_hd * col, cudaMemcpyHostToDevice, st));
+    if (fields && h->nf)
+        CU(h, cudaMemcpyAsync(kriged_values(h), h->hfields.data(), h->nf * col, cudaMemcpyHostToDevice, st));
+    for (double* a : {b.ax, b.ay, b.az}) CU(h, cudaMemsetAsync(a, 0, (size_t)h->n_pad * 8, st));
+    CU(h, kbk_adjust_data(h->dim, h->an, h->n, raw_col(h, RAW_X), raw_col(h, RAW_Y), raw_col(h, RAW_Z),
+                          b.ax, b.ay, b.az, st)); ++*launches;
+    CU(h, cudaEventRecord(h->ev[EV_ADJUSTED], st));
+    return KB200_OK;
+}
+
+// The three factorisations of kb200_set_problem. Each returns the gform of its tiles (or an error code < 0); the
+// flag it leaves in wFlag is non-zero when the drift/unbiasedness block is singular.
+
+// pseudo_inv=True: A^+ of the bordered gamma-form matrix (pinv.cu), then the quadratic-form solve
+static int factor_pinv(kb200_ctx* h, const BlobView& b, int* launches) {
+    cudaStream_t st = h->stream;
+    const int nn = h->n, np = h->n_pad, nt = nn + h->K1;
+    double* Fz = aux_block(h, AUX_F);
+    double* Uz = aux_block(h, AUX_U);
+    int* flag = h->wFlag.as<int>();
+    CU(h, h->wVario.reserve(kbk_pinv_workspace_doubles(nt) * sizeof(double)));
+    CU(h, cudaEventRecord(h->ev[EV_INVERT], st));
+    CU(h, kbk_build_fz(nn, np, h->n_rl, h->n_hd, b.ax, b.ay, b.az, h->ds, raw_col(h, RAW_DRIFT), raw_col(h, RAW_V), Fz,
+                       st)); ++*launches;
+    CU(h, kbk_pinv(nn, h->K1, np, h->wC.as<double>(), h->ld, Fz, raw_col(h, RAW_V), Uz, b.consts, h->wVario.as<double>(),
+                   flag, st, launches, &h->pinv_sweeps, &h->pinv_rank));
+    if (h->pinv_sweeps < 0) { h->launches += *launches; return fail(h, KB200_ESINGULAR, "pseudo-inverse: the Jacobi SVD did not converge"); }
+    CU(h, cudaMemsetAsync(flag, 0, sizeof(int), st));
+    CU(h, cudaEventRecord(h->ev[EV_DUAL], st));
+    CU(h, kbk_pack_gform(h->wC.as<double>(), h->ld, nn, np, h->na, Uz, h->pm, b.tiles, st)); ++*launches;
+    return 2;
+}
+
+// C is not positive definite: the variogram is not conditionally negative definite in this dimension (e.g. hole-effect
+// on dense scatter). General fallback, from the unshifted c0: blocked Gauss-Jordan inverse with partial pivoting +
+// quadratic-form solve (DESIGN.md §3b). fp64 only.
+static int factor_general(kb200_ctx* h, const BlobView& b, double c0, float* t_chol, int* launches) {
+    if (h->dtype != KB200_F64) {
+        h->launches += *launches;
+        return fail(h, KB200_EUNSUPPORTED, "dtype float32 / float64x need a positive definite covariance form "
+                    "(the variogram is not valid in this dimension); use float64");
+    }
+    cudaStream_t st = h->stream;
+    const int nn = h->n, np = h->n_pad, ld = h->ld;
+    double* G = h->wC.as<double>();
+    int* flag = h->wFlag.as<int>();
+    h->vg.c0 = c0;
+    CU(h, cudaMemsetAsync(flag, 0, sizeof(int), st));
+    CU(h, cudaEventRecord(h->ev[EV_FACTOR], st));
+    CU(h, kbk_assemble(h->dim, h->vg, nn, np, ld, b.ax, b.ay, b.az, G, st)); ++*launches;
+    CU(h, h->wVario.reserve(kbk_general_inverse_workspace_bytes(np)));
+    const char* gj_env = std::getenv("KB200_GJ");            // "scalar": the tests' cross-check of the blocked default
+    CU(h, kbk_general_inverse(G, ld, nn, np, h->wVario.p, flag, 3.6e-15 * h->vg.c0, st, launches,
+                              gj_env && gj_env[0] == 's'));
+    CU(h, cudaEventRecord(h->ev[EV_INVERT], st));
+    int hflag = 0;
+    CU(h, cudaMemcpyAsync(&hflag, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    *t_chol += ev_ms(h->ev[EV_FACTOR], h->ev[EV_INVERT]);
+    if (hflag != 0) {
+        h->launches += *launches;
+        return fail(h, KB200_ESINGULAR, "kriging matrix is singular (zero pivot in column " +
+                    std::to_string(hflag - 1) + ")");
+    }
+    double* Uz = aux_block(h, AUX_U);
+    CU(h, cudaEventRecord(h->ev[EV_DUAL], st));
+    CU(h, kbk_dual_gform(G, ld, nn, np, h->n_rl, h->n_hd, h->nf ? h->nf : 1, b.ax, b.ay, b.az, h->ds,
+                         raw_col(h, RAW_DRIFT), kriged_values(h), aux_block(h, AUX_F), Uz, b.consts, flag, st, launches));
+    CU(h, kbk_pack_gform(G, ld, nn, np, h->na, Uz, h->pm, b.tiles, st)); ++*launches;
+    return 1;
+}
+
+// C = L L^T (L in wC): W = L^-1, the dual vectors, and W packed into the tiles of the handle's dtype
+static int factor_cholesky_pack(kb200_ctx* h, const BlobView& b, int* launches) {
+    cudaStream_t st = h->stream;
+    const int nn = h->n, np = h->n_pad, ld = h->ld;
+    double* W = h->wW.as<double>();
+    double* Uz = aux_block(h, AUX_U);
+    CU(h, kbk_trtri(h->wC.as<double>(), W, h->wT.as<double>(), ld, np, st, launches));
+    CU(h, cudaEventRecord(h->ev[EV_DUAL], st));
+    CU(h, kbk_dual(W, ld, nn, np, h->n_rl, h->n_hd, h->nf ? h->nf : 1, b.ax, b.ay, b.az, h->ds, raw_col(h, RAW_DRIFT),
+                   kriged_values(h), aux_block(h, AUX_F), aux_block(h, AUX_H), Uz, b.consts, h->wFlag.as<int>(), st,
+                   launches));
+    if (h->dtype == KB200_F32) {
+        CU(h, kbk_pack_tf32(W, ld, nn, np, h->na, Uz, h->pm, b.tiles, st)); ++*launches;
+    } else if (h->slices) {
+        const int nrb8 = kbk_i8_nrb(h->slices, nn, h->na);
+        std::vector<long long> toff(nrb8 + 1);
+        kbk_i8_total_tiles(h->slices, nn, h->na, toff.data());
+        // workspace (T1 scratch is free now): tile offsets | row exponents
+        long long* d_toff = reinterpret_cast<long long*>(h->wT.as<char>());
+        int* d_rowexp = reinterpret_cast<int*>(h->wT.as<char>() + align_up((size_t)(nrb8 + 1) * sizeof(long long), 256));   // kbk_i8_rows ints
+        CU(h, cudaMemcpyAsync(d_toff, toff.data(), (size_t)(nrb8 + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
+        CU(h, kbk_pack_i8(h->slices, W, ld, nn, np, h->na, Uz, d_rowexp, b.rowscale, d_toff, b.tiles, st));
+        *launches += 2;                        // row scales + pack
+        CU(h, cudaStreamSynchronize(st));      // toff is a host temporary
+    } else {
+        CU(h, kbk_pack(h->dtype, W, ld, nn, np, h->na, Uz, h->pm, b.tiles, st)); ++*launches;
+    }
+    return 0;
+}
 
 extern "C" int kb200_set_problem(kb200_handle h, int dim, int dtype, int64_t n,
                                  const double* x, const double* y, const double* z, const double* values,
@@ -461,33 +630,11 @@ extern "C" int kb200_set_problem(kb200_handle h, int dim, int dtype, int64_t n,
     const size_t mat = (size_t)np * ld * sizeof(double);
     CU(h, h->wC.reserve(mat)); CU(h, h->wW.reserve(mat)); CU(h, h->wT.reserve(mat));
     CU(h, h->wF.reserve((size_t)3 * h->aux_cols * np * sizeof(double)));
-    CU(h, h->wRaw.reserve((size_t)(4 + h->n_hd + h->nf) * nn * sizeof(double)));
     CU(h, h->wFlag.reserve(256));
-    double* raw = h->wRaw.as<double>();
-    double *rx = raw, *ry = raw + nn, *rz = raw + 2 * (size_t)nn, *rv = raw + 3 * (size_t)nn, *rh = raw + 4 * (size_t)nn;
-    double* rf = rh + (size_t)h->n_hd * nn;          // value fields: nf columns of nn
-    const int nv = h->nf ? h->nf : 1;
-    const double* vals = h->nf ? rf : rv;
-    char* blob = h->blob.as<char>();
-    double* ax = reinterpret_cast<double*>(blob + h->off_ax);
-    double* ay = reinterpret_cast<double*>(blob + h->off_ay);
-    double* az = reinterpret_cast<double*>(blob + h->off_az);
-    double* consts = reinterpret_cast<double*>(blob + h->off_consts);
+    const BlobView b = blob_view(h);
     int* flag = h->wFlag.as<int>();
     int launches = 0;
-
-    CU(h, cudaEventRecord(h->ev[0], st));
-    CU(h, cudaMemcpyAsync(rx, h->hx.data(), nn * 8, cudaMemcpyHostToDevice, st));
-    CU(h, cudaMemcpyAsync(ry, h->hy.data(), nn * 8, cudaMemcpyHostToDevice, st));
-    CU(h, cudaMemcpyAsync(rz, h->hz.data(), nn * 8, cudaMemcpyHostToDevice, st));
-    CU(h, cudaMemcpyAsync(rv, h->hval.data(), nn * 8, cudaMemcpyHostToDevice, st));
-    if (h->n_hd) CU(h, cudaMemcpyAsync(rh, h->hdrift.data(), (size_t)h->n_hd * nn * 8, cudaMemcpyHostToDevice, st));
-    if (h->nf) CU(h, cudaMemcpyAsync(rf, h->hfields.data(), (size_t)h->nf * nn * 8, cudaMemcpyHostToDevice, st));
-    CU(h, cudaMemsetAsync(ax, 0, (size_t)np * 8, st));
-    CU(h, cudaMemsetAsync(ay, 0, (size_t)np * 8, st));
-    CU(h, cudaMemsetAsync(az, 0, (size_t)np * 8, st));
-    CU(h, kbk_adjust_data(h->dim, h->an, nn, rx, ry, rz, ax, ay, az, st)); ++launches;
-    CU(h, cudaEventRecord(h->ev[1], st));
+    rc = upload_data(h, true, &launches); if (rc) return rc;
 
     // covariance shift: c0 = sill for bounded models; for linear/power grow c0 until C is
     // positive definite (DESIGN.md §3). A model that is not a valid variogram in this
@@ -499,128 +646,56 @@ extern "C" int kb200_set_problem(kb200_handle h, int dim, int dtype, int64_t n,
     float t_asm = 0.f, t_chol = 0.f;
     for (int attempt = 0; attempt < max_try; ++attempt) {
         CU(h, cudaMemsetAsync(flag, 0, sizeof(int), st));
-        CU(h, cudaEventRecord(h->ev[2], st));
-        CU(h, kbk_assemble(h->dim, h->vg, nn, np, ld, ax, ay, az, h->wC.as<double>(), st)); ++launches;
-        CU(h, cudaEventRecord(h->ev[3], st));
+        CU(h, cudaEventRecord(h->ev[EV_ASM], st));
+        CU(h, kbk_assemble(h->dim, h->vg, nn, np, ld, b.ax, b.ay, b.az, h->wC.as<double>(), st)); ++launches;
+        CU(h, cudaEventRecord(h->ev[EV_FACTOR], st));
         if (h->pinv) {                                  // no factorisation: the pseudo-inverse works on -Gamma itself
-            CU(h, cudaEventRecord(h->ev[4], st));
+            CU(h, cudaEventRecord(h->ev[EV_INVERT], st));
             CU(h, cudaStreamSynchronize(st));
-            t_asm += ev_ms(h->ev[2], h->ev[3]);
+            t_asm += ev_ms(h->ev[EV_ASM], h->ev[EV_FACTOR]);
             break;
         }
-        {
-            if (!h->hi_stream) {
-                int lo = 0, hi = 0;
-                CU(h, cudaDeviceGetStreamPriorityRange(&lo, &hi));
-                CU(h, cudaStreamCreateWithPriority(&h->hi_stream, cudaStreamNonBlocking, hi));
-            }
-            const size_t need = 2 * (size_t)((np / 64 + 3) / 4) + 1;
-            while (h->fev.size() < need) {
-                cudaEvent_t e;
-                CU(h, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-                h->fev.push_back(e);
-            }
+        if (!h->hi_stream) {
+            int lo = 0, hi = 0;
+            CU(h, cudaDeviceGetStreamPriorityRange(&lo, &hi));
+            CU(h, cudaStreamCreateWithPriority(&h->hi_stream, cudaStreamNonBlocking, hi));
+        }
+        const size_t need = 2 * (size_t)((np / 64 + 3) / 4) + 1;
+        while (h->fev.size() < need) {
+            cudaEvent_t e;
+            CU(h, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+            h->fev.push_back(e);
         }
         CU(h, kbk_cholesky(h->wC.as<double>(), h->wW.as<double>(), h->wT.as<double>(), ld, np, flag, 3.6e-15 * h->vg.c0, st, h->hi_stream,
                            h->fev.data(), (int)h->fev.size(), &launches));
-        CU(h, cudaEventRecord(h->ev[4], st));
+        CU(h, cudaEventRecord(h->ev[EV_INVERT], st));
         CU(h, cudaMemcpyAsync(&hflag, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
         CU(h, cudaStreamSynchronize(st));
-        t_asm += ev_ms(h->ev[2], h->ev[3]); t_chol += ev_ms(h->ev[3], h->ev[4]);
+        t_asm += ev_ms(h->ev[EV_ASM], h->ev[EV_FACTOR]); t_chol += ev_ms(h->ev[EV_FACTOR], h->ev[EV_INVERT]);
         if (hflag != 0 && std::getenv("KB200_DEBUG")) std::fprintf(stderr, "[kb200] cholesky flag %d (attempt %d, c0 %g)\n", hflag, attempt, h->vg.c0);
         if (hflag == 0) break;
         h->vg.c0 *= 2.0;
     }
-    h->gform = 0;
-    double* Fz = h->wF.as<double>();
-    double* Hz = Fz + (size_t)h->aux_cols * np;
-    double* Uz = Hz + (size_t)h->aux_cols * np;
-    CU(h, cudaMemsetAsync(consts, 0, (size_t)std::max(512, h->K1 * h->na) * sizeof(double), st));
-    if (h->pinv) {
-        // pseudo_inv=True: A^+ of the bordered gamma-form matrix (pinv.cu), then the quadratic-form solve
-        const int nt = nn + h->K1;
-        CU(h, h->wVario.reserve(kbk_pinv_workspace_doubles(nt) * sizeof(double)));
-        CU(h, cudaEventRecord(h->ev[4], st));
-        CU(h, kbk_build_fz(nn, np, h->n_rl, h->n_hd, ax, ay, az, h->ds, rh, rv, Fz, st)); ++launches;
-        CU(h, kbk_pinv(nn, h->K1, np, h->wC.as<double>(), ld, Fz, rv, Uz, consts, h->wVario.as<double>(), flag, st,
-                       &launches, &h->pinv_sweeps, &h->pinv_rank));
-        if (h->pinv_sweeps < 0) { h->launches += launches; return fail(h, KB200_ESINGULAR, "pseudo-inverse: the Jacobi SVD did not converge"); }
-        CU(h, cudaMemsetAsync(flag, 0, sizeof(int), st));
-        CU(h, cudaEventRecord(h->ev[5], st));
-        CU(h, kbk_pack_gform(h->wC.as<double>(), ld, nn, np, h->na, Uz, h->pm, blob + h->off_tiles, st)); ++launches;
-        h->gform = 2;
-    } else if (hflag != 0) {
-        // C is not positive definite: the variogram is not conditionally negative definite in this
-        // dimension (e.g. hole-effect on dense scatter). General fallback: blocked Gauss-Jordan inverse with
-        // partial pivoting + quadratic-form solve (DESIGN.md §3b). fp64 only.
-        if (h->dtype != KB200_F64) {
-            h->launches += launches;
-            return fail(h, KB200_EUNSUPPORTED, "dtype float32 / float64x need a positive definite covariance form "
-                        "(the variogram is not valid in this dimension); use float64");
-        }
-        h->vg.c0 = c0_first;
-        CU(h, cudaMemsetAsync(flag, 0, sizeof(int), st));
-        CU(h, cudaEventRecord(h->ev[3], st));
-        CU(h, kbk_assemble(h->dim, h->vg, nn, np, ld, ax, ay, az, h->wC.as<double>(), st)); ++launches;
-        CU(h, h->wVario.reserve(kbk_general_inverse_workspace_bytes(np)));
-        const char* gj_env = std::getenv("KB200_GJ");            // "blocked" | "scalar": cross-check switch of the tests
-        const bool gj_scalar = gj_env ? gj_env[0] == 's' : !KB_GJ_DEFAULT_BLOCKED;
-        CU(h, kbk_general_inverse(h->wC.as<double>(), ld, nn, np, h->wVario.p, flag, 3.6e-15 * h->vg.c0, st, &launches,
-                                  gj_scalar));
-        CU(h, cudaEventRecord(h->ev[4], st));
-        CU(h, cudaMemcpyAsync(&hflag, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
-        CU(h, cudaStreamSynchronize(st));
-        t_chol += ev_ms(h->ev[3], h->ev[4]);
-        if (hflag != 0) {
-            h->launches += launches;
-            return fail(h, KB200_ESINGULAR, "kriging matrix is singular (zero pivot in column " +
-                        std::to_string(hflag - 1) + ")");
-        }
-        h->gform = 1;
-        CU(h, cudaEventRecord(h->ev[5], st));
-        CU(h, kbk_dual_gform(h->wC.as<double>(), ld, nn, np, h->n_rl, h->n_hd, nv, ax, ay, az, h->ds, rh, vals,
-                             Fz, Uz, consts, flag, st, &launches));
-        CU(h, kbk_pack_gform(h->wC.as<double>(), ld, nn, np, h->na, Uz, h->pm, blob + h->off_tiles, st)); ++launches;
-    } else {
-    CU(h, kbk_trtri(h->wC.as<double>(), h->wW.as<double>(), h->wT.as<double>(), ld, np, st, &launches));
-    CU(h, cudaEventRecord(h->ev[5], st));
-    CU(h, kbk_dual(h->wW.as<double>(), ld, nn, np, h->n_rl, h->n_hd, nv, ax, ay, az, h->ds, rh, vals,
-                   Fz, Hz, Uz, consts, flag, st, &launches));
-    if (h->dtype == KB200_F32) {
-        CU(h, kbk_pack_tf32(h->wW.as<double>(), ld, nn, np, h->na, Uz, h->pm, blob + h->off_tiles, st));
-    } else if (h->slices) {
-        const int nrb8 = kbk_i8_nrb(h->slices, nn, h->na);
-        std::vector<long long> toff(nrb8 + 1);
-        kbk_i8_total_tiles(h->slices, nn, h->na, toff.data());
-        // workspace (T1 scratch is free now): tile offsets | row exponents
-        long long* d_toff = reinterpret_cast<long long*>(h->wT.as<char>());
-        int* d_rowexp = reinterpret_cast<int*>(h->wT.as<char>() + align_up((size_t)(nrb8 + 1) * sizeof(long long), 256));   // kbk_i8_rows ints
-        CU(h, cudaMemcpyAsync(d_toff, toff.data(), (size_t)(nrb8 + 1) * sizeof(long long), cudaMemcpyHostToDevice, st));
-        CU(h, kbk_pack_i8(h->slices, h->wW.as<double>(), ld, nn, np, h->na, Uz, d_rowexp,
-                          reinterpret_cast<double*>(blob + h->off_rowscale), d_toff, blob + h->off_tiles, st));
-        CU(h, cudaStreamSynchronize(st));      // toff is a host temporary
-        ++launches;
-    } else {
-        CU(h, kbk_pack(h->dtype, h->wW.as<double>(), ld, nn, np, h->na, Uz, h->pm, blob + h->off_tiles, st));
-    }
-    ++launches;
-    }
-    double hdr[64] = {0};
-    hdr[0] = KB_MAGIC; hdr[1] = h->vg.c0; hdr[34] = (double)h->gform;
-    for (int c = 0; c <= KB200_MAX_DRIFT; ++c) { hdr[2 + c] = h->ds.shift[c]; hdr[18 + c] = h->ds.scale[c]; }
-    CU(h, cudaMemcpyAsync(blob, hdr, sizeof(hdr), cudaMemcpyHostToDevice, st));
-    CU(h, cudaEventRecord(h->ev[6], st));
+    CU(h, cudaMemsetAsync(b.consts, 0, (size_t)std::max(512, h->K1 * h->na) * sizeof(double), st));
+    const int gform = h->pinv ? factor_pinv(h, b, &launches)
+                    : hflag ? factor_general(h, b, c0_first, &t_chol, &launches)
+                    : factor_cholesky_pack(h, b, &launches);
+    if (gform < 0) return gform;
+    h->gform = gform;
+    double hdr[HDR_DOUBLES];
+    write_header(h, hdr);
+    CU(h, cudaMemcpyAsync(b.hdr, hdr, sizeof(hdr), cudaMemcpyHostToDevice, st));
+    CU(h, cudaEventRecord(h->ev[EV_PACKED], st));
     CU(h, cudaMemcpyAsync(&hflag, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
     CU(h, cudaStreamSynchronize(st));
-    h->tm[6] += ev_ms(h->ev[0], h->ev[1]);
-    h->tm[0] += t_asm; h->tm[1] += t_chol;
-    h->tm[2] += ev_ms(h->ev[4], h->ev[5]);
-    h->tm[3] += ev_ms(h->ev[5], h->ev[6]);
+    h->tm[TM_H2D] += ev_ms(h->ev[EV_UPLOAD], h->ev[EV_ADJUSTED]);
+    h->tm[TM_ASSEMBLE] += t_asm; h->tm[TM_CHOLESKY] += t_chol;
+    h->tm[TM_TRTRI] += ev_ms(h->ev[EV_INVERT], h->ev[EV_DUAL]);
+    h->tm[TM_PACK_DUAL] += ev_ms(h->ev[EV_DUAL], h->ev[EV_PACKED]);
     h->launches += launches;
     if (hflag != 0) return fail(h, KB200_ESINGULAR, "drift/unbiasedness block F^T C^-1 F is singular");
     h->ready = true;
-    h->factor_live = !h->gform;
-    h->inv_live = h->gform != 2;
+    h->local_factor = true;
     return KB200_OK;
 }
 
@@ -634,7 +709,7 @@ extern "C" int kb200_set_device_drift(kb200_handle h, int n_wells, const double*
     const bool ext = ext_nx > 0 || ext_ny > 0;
     if (ext && (ext_nx < 1 || ext_ny < 1 || ext_nx > (1 << 30) || ext_ny > (1 << 30) || !ext_x || !ext_y || !ext_z))
         return fail(h, KB200_EBADARG, "device drift: bad external_Z raster description");
-    h->described = false; h->ready = false; h->factor_live = false;
+    drop_problem(h);
     cudaSetDevice(h->device);
     h->dd = DeviceDrift{};
     if (n_wells) {
@@ -660,18 +735,12 @@ extern "C" int kb200_set_device_drift(kb200_handle h, int n_wells, const double*
 }
 
 // ---- execute --------------------------------------------------------------
-// One persistent launch of the solve kernel of the handle's dtype over points [s.first, s.first + s.count).
-// NOTE: one kernel for every point count: the summation order per point must not depend on how the points are
-// sharded or chunked (concatenated shards == single call, bit for bit; SURVEY.md §4 (iii)).
 // One persistent launch of the solve kernel of the handle's dtype over points [s.first, s.first + s.count) with point
-// tiles of `tp` points.
+// tiles of `tp` points. One kernel serves every point count: the summation order per point must not depend on how the
+// points are sharded or chunked (concatenated shards == single call, bit for bit; SURVEY.md §4 (iii)).
 static int launch_solve(kb200_ctx* h, const Src& s, double* d_z, double* d_ss, int tp) {
     cudaStream_t st = h->stream;
-    char* blob = h->blob.as<char>();
-    PointSource ps{};
-    ps.grid = s.grid ? 1 : 0;
-    ps.px = s.a; ps.py = s.b; ps.pz = s.c; ps.gx = s.a; ps.gy = s.b; ps.gz = s.c;
-    ps.nx = s.nx; ps.ny = s.ny; ps.nz = s.nz;
+    const BlobView b = blob_view(h);
     const bool i8 = h->slices != 0;
     const bool f32 = h->dtype == KB200_F32;
     long long ntiles = (s.count + tp - 1) / tp;
@@ -679,13 +748,11 @@ static int launch_solve(kb200_ctx* h, const Src& s, double* d_z, double* d_ss, i
     CU(h, h->wScratch.reserve(i8 ? kbk_solve_i8_scratch_bytes(h->slices, h->n, grid) : f32 ? kbk_solve_tf32_scratch_bytes(h->n, grid)
                                   : kbk_solve_pt_scratch_doubles(h->n, grid) * sizeof(double)));
     SolvePtParams pp{};
-    pp.vg = h->vg; pp.an = h->an; ps.first = s.first; pp.ps = ps;
+    pp.vg = h->vg; pp.an = h->an; pp.ps = s.point_source();
     pp.n = h->n; pp.na = h->na; pp.nrb = h->nrb; pp.n_rl = h->n_rl; pp.n_hd = h->n_hd;
-    pp.ax = reinterpret_cast<double*>(blob + h->off_ax);
-    pp.ay = reinterpret_cast<double*>(blob + h->off_ay);
-    pp.az = reinterpret_cast<double*>(blob + h->off_az);
-    pp.tiles = blob + h->off_tiles; pp.pm = h->pm; pp.ds = h->ds;
-    pp.consts = reinterpret_cast<double*>(blob + h->off_consts);
+    pp.ax = b.ax; pp.ay = b.ay; pp.az = b.az;
+    pp.tiles = b.tiles; pp.pm = h->pm; pp.ds = h->ds;
+    pp.consts = b.consts;
     pp.dd = h->dd; pp.n_dev = h->n_dev;
     pp.drift_pts = s.d_drift; pp.drift_stride = s.drift_stride; pp.drift_first = s.drift_first;
     pp.m = s.count; pp.scratch = h->wScratch.as<double>(); pp.gform = h->gform;
@@ -695,7 +762,7 @@ static int launch_solve(kb200_ctx* h, const Src& s, double* d_z, double* d_ss, i
         CU(h, h->wFstage.reserve((size_t)grid * h->na * tp * sizeof(double)));
         pp.fstage = h->wFstage.as<double>();
     }
-    pp.rowscale = reinterpret_cast<const double*>(blob + h->off_rowscale);
+    pp.rowscale = b.rowscale;
     if (i8) CU(h, kbk_solve_i8(h->slices, h->dim, pp, grid, st));
     else if (f32) CU(h, kbk_solve_tf32(h->dim, pp, grid, st));
     else CU(h, kbk_solve_pt(h->dim, pp, grid, tp, st));
@@ -707,8 +774,8 @@ static int launch_solve(kb200_ctx* h, const Src& s, double* d_z, double* d_ss, i
 // width; the DMMA work is proportional to the width), at N=5000 (scripts/tile_timing.py).
 static double tile_cost(int tp) { return tp == 64 ? 1.0 : (tp == 32 ? KB_TILE_COST_32 : KB_TILE_COST_16); }
 
-// NOTE: the summation order per point does not depend on the tile width, on how the points are sharded or chunked, or on
-// the number of launches (concatenated shards == single call, bit for bit; SURVEY.md §4 (iii)).
+// NOTE: the summation order per point does not depend on the tile width or on the number of launches either, so the
+// split below is free to choose them.
 static int run_solve(kb200_ctx* h, const Src& s, double* d_z, double* d_ss) {
     const bool i8 = h->slices != 0;
     const bool f32 = h->dtype == KB200_F32;
@@ -725,8 +792,7 @@ static int run_solve(kb200_ctx* h, const Src& s, double* d_z, double* d_ss) {
     const long long main_pts = std::min<long long>(s.count, (nt64 / S) * S * TW);
     const long long rem = s.count - main_pts;
     if (main_pts > 0) {
-        Src m = s; m.count = main_pts;
-        int rc = launch_solve(h, m, d_z, d_ss, TW); if (rc) return rc;
+        int rc = launch_solve(h, s.sub(0, main_pts), d_z, d_ss, TW); if (rc) return rc;
     }
     if (rem > 0) {
         int best = TW; double bc = 1e300;
@@ -736,13 +802,10 @@ static int run_solve(kb200_ctx* h, const Src& s, double* d_z, double* d_ss) {
             const double c = (double)((nt + S - 1) / S) * tile_cost(tp);
             if (c < bc * 0.999) { bc = c; best = tp; }
         }
-        Src t = s; t.first = s.first + main_pts; t.count = rem; t.drift_first = s.drift_first + main_pts;
-        int rc = launch_solve(h, t, d_z + main_pts, d_ss + main_pts, best); if (rc) return rc;
+        int rc = launch_solve(h, s.sub(main_pts, rem), d_z + main_pts, d_ss + main_pts, best); if (rc) return rc;
     }
     return KB200_OK;
 }
-
-static int run_knn(kb200_ctx* h, int k, const Src& s, double* d_z, double* d_ss, int chol, int loo = 0);
 
 // Launch `total` points in chunks and bring (z, ss) to the caller's HOST buffers. Large outputs travel through two
 // pinned staging buffers on a second stream while the next chunk computes; the host drains a buffer into the
@@ -756,15 +819,15 @@ static int run_to_host(kb200_ctx* h, int64_t total, double* z_out, double* ss_ou
     CU(h, h->wOut.reserve((size_t)(nzb + 1) * total * 8));
     double* dz = h->wOut.as<double>();
     double* dss = dz + (size_t)nzb * total;
-    CU(h, cudaEventRecord(h->ev[7], st));
+    CU(h, cudaEventRecord(h->ev[EV_RUN], st));
     if (total < KB_STAGE_MIN) {
         int rc = launch((int64_t)0, total, dz, dss); if (rc) return rc;
-        CU(h, cudaEventRecord(h->ev[8], st));
+        CU(h, cudaEventRecord(h->ev[EV_RUN_END], st));
         CU(h, cudaMemcpyAsync(z_out, dz, (size_t)nzb * total * 8, cudaMemcpyDeviceToHost, st));
         CU(h, cudaMemcpyAsync(ss_out, dss, total * 8, cudaMemcpyDeviceToHost, st));
-        CU(h, cudaEventRecord(h->ev[11], st));
+        CU(h, cudaEventRecord(h->ev[EV_D2H_END], st));
         CU(h, cudaStreamSynchronize(st));
-        h->tm[7] += ev_ms(h->ev[8], h->ev[11]);
+        h->tm[TM_D2H] += ev_ms(h->ev[EV_RUN_END], h->ev[EV_D2H_END]);
         return KB200_OK;
     }
     if (!h->copy_stream) {
@@ -798,7 +861,7 @@ static int run_to_host(kb200_ctx* h, int64_t total, double* z_out, double* ss_ou
         const int64_t o = c * KB_STAGE_PTS, m = chunk_len(c);
         int rc = launch(o, m, dz + o, dss + o); if (rc) return rc;
         CU(h, cudaEventRecord(h->evk[b], st));
-        if (c == nch - 1) CU(h, cudaEventRecord(h->ev[8], st));
+        if (c == nch - 1) CU(h, cudaEventRecord(h->ev[EV_RUN_END], st));
         if (c >= 2) { rc = drain(c - 2); if (rc) return rc; }
         double* p = reinterpret_cast<double*>(h->pin[b]);
         CU(h, cudaStreamWaitEvent(h->copy_stream, h->evk[b], 0));
@@ -810,7 +873,7 @@ static int run_to_host(kb200_ctx* h, int64_t total, double* z_out, double* ss_ou
     }
     for (int64_t c = std::max<int64_t>(0, nch - 2); c < nch; ++c) { int rc = drain(c); if (rc) return rc; }
     CU(h, cudaStreamSynchronize(st));
-    h->tm[7] += ev_ms(h->ev[8], h->evc[(nch - 1) & 1]);
+    h->tm[TM_D2H] += ev_ms(h->ev[EV_RUN_END], h->evc[(nch - 1) & 1]);
     return KB200_OK;
 }
 
@@ -822,28 +885,40 @@ static int check_ready(kb200_ctx* h) {
 }
 static int n_host_drift(const kb200_ctx* h) { return h->n_hd - h->n_dev; }
 
-extern "C" int kb200_execute_points_dev(kb200_handle h, int64_t m,
-                                        const double* d_px, const double* d_py, const double* d_pz,
-                                        const double* d_drift_pts, double* d_z, double* d_ss) {
-    int rc = check_ready(h); if (rc) return rc;
-    if (m <= 0) return KB200_OK;
-    if (!d_px || !d_py || (h->dim == 3 && !d_pz) || !d_z || !d_ss) return fail(h, KB200_EBADARG, "null pointer");
-    if (n_host_drift(h) && !d_drift_pts) return fail(h, KB200_EBADARG, "drift values at the points are required");
-    Src s{false, 0, 0, 0, d_px, d_py, d_pz, 0, m, d_drift_pts, m, 0};
-    h->zstride = m;
-    CU(h, cudaEventRecord(h->ev[7], h->stream));
-    rc = run_solve(h, s, d_z, d_ss); if (rc) return rc;
-    CU(h, cudaEventRecord(h->ev[8], h->stream));
-    CU(h, cudaStreamSynchronize(h->stream));
-    h->tm[4] += ev_ms(h->ev[7], h->ev[8]);
-    return KB200_OK;
-}
-
 static int check_grid(kb200_ctx* h, int64_t nx, int64_t ny, int64_t nz, int64_t first, int64_t count) {
     if (nx < 1 || ny < 1 || nz < 1 || first < 0 || count < 0 || first + count > nx * ny * nz)
         return fail(h, KB200_EBADARG, "bad grid slice");
     if (h->dim != 3 && nz != 1) return fail(h, KB200_EBADARG, "nz must be 1 for 2-D");
     return KB200_OK;
+}
+
+// the caller's arrays of an execute call: the points or axes, the outputs and (if the problem has host drift columns)
+// the drift values at the points
+static int check_io(kb200_ctx* h, const double* a, const double* b, const double* c, const double* drift,
+                    const double* z, const double* ss) {
+    if (!a || !b || (h->dim == 3 && !c) || !z || !ss) return fail(h, KB200_EBADARG, "null pointer");
+    if (n_host_drift(h) && !drift) return fail(h, KB200_EBADARG, "drift values at the points are required");
+    return KB200_OK;
+}
+
+// the global solve of points already on the device, into the caller's device buffers
+static int solve_dev(kb200_ctx* h, const Src& s, double* d_z, double* d_ss) {
+    if (s.count <= 0) return KB200_OK;
+    int rc = check_io(h, s.a, s.b, s.c, s.d_drift, d_z, d_ss); if (rc) return rc;
+    h->zstride = s.count;
+    CU(h, cudaEventRecord(h->ev[EV_RUN], h->stream));
+    rc = run_solve(h, s, d_z, d_ss); if (rc) return rc;
+    CU(h, cudaEventRecord(h->ev[EV_RUN_END], h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
+    h->tm[TM_SOLVE] += ev_ms(h->ev[EV_RUN], h->ev[EV_RUN_END]);
+    return KB200_OK;
+}
+
+extern "C" int kb200_execute_points_dev(kb200_handle h, int64_t m,
+                                        const double* d_px, const double* d_py, const double* d_pz,
+                                        const double* d_drift_pts, double* d_z, double* d_ss) {
+    int rc = check_ready(h); if (rc) return rc;
+    return solve_dev(h, Src{false, 0, 0, 0, d_px, d_py, d_pz, 0, m, d_drift_pts, m, 0}, d_z, d_ss);
 }
 
 extern "C" int kb200_execute_grid_dev(kb200_handle h, int64_t nx, int64_t ny, int64_t nz,
@@ -852,104 +927,7 @@ extern "C" int kb200_execute_grid_dev(kb200_handle h, int64_t nx, int64_t ny, in
                                       double* d_z, double* d_ss) {
     int rc = check_ready(h); if (rc) return rc;
     rc = check_grid(h, nx, ny, nz, first, count); if (rc) return rc;
-    if (count == 0) return KB200_OK;
-    if (!d_gx || !d_gy || (h->dim == 3 && !d_gz) || !d_z || !d_ss) return fail(h, KB200_EBADARG, "null pointer");
-    if (n_host_drift(h) && !d_drift_pts) return fail(h, KB200_EBADARG, "drift values at the points are required");
-    Src s{true, nx, ny, nz, d_gx, d_gy, d_gz, first, count, d_drift_pts, count, 0};
-    h->zstride = count;
-    CU(h, cudaEventRecord(h->ev[7], h->stream));
-    rc = run_solve(h, s, d_z, d_ss); if (rc) return rc;
-    CU(h, cudaEventRecord(h->ev[8], h->stream));
-    CU(h, cudaStreamSynchronize(h->stream));
-    h->tm[4] += ev_ms(h->ev[7], h->ev[8]);
-    return KB200_OK;
-}
-
-// host drift columns [n_host][stride] -> device columns [n_host][m] holding items [off, off + m) of each column
-static int upload_drift(kb200_ctx* h, const double* drift_pts, int64_t stride, int64_t off, int64_t m, const double** dd) {
-    *dd = nullptr;
-    const int nh = n_host_drift(h);
-    if (!nh) return KB200_OK;
-    CU(h, h->wDrift.reserve((size_t)nh * m * 8));
-    for (int c = 0; c < nh; ++c)
-        CU(h, cudaMemcpyAsync(h->wDrift.as<double>() + (size_t)c * m, drift_pts + (size_t)c * stride + off, (size_t)m * 8,
-                              cudaMemcpyHostToDevice, h->stream));
-    *dd = h->wDrift.as<double>();
-    return KB200_OK;
-}
-
-// points [off, off + m) of the caller's arrays (drift columns have `stride` items each)
-static int exec_points_impl(kb200_ctx* h, int64_t off, int64_t m, const double* px, const double* py, const double* pz,
-                            const double* drift_pts, int64_t stride, double* z_out, double* ss_out) {
-    int rc = check_ready(h); if (rc) return rc;
-    if (m <= 0) return KB200_OK;
-    if (!px || !py || (h->dim == 3 && !pz) || !z_out || !ss_out) return fail(h, KB200_EBADARG, "null pointer");
-    if (n_host_drift(h) && !drift_pts) return fail(h, KB200_EBADARG, "drift values at the points are required");
-    cudaStream_t st = h->stream;
-    CU(h, h->wPts.reserve((size_t)3 * m * 8));
-    double* dp = h->wPts.as<double>();
-    CU(h, cudaEventRecord(h->ev[9], st));
-    CU(h, cudaMemcpyAsync(dp, px + off, m * 8, cudaMemcpyHostToDevice, st));
-    CU(h, cudaMemcpyAsync(dp + m, py + off, m * 8, cudaMemcpyHostToDevice, st));
-    if (h->dim == 3) CU(h, cudaMemcpyAsync(dp + 2 * m, pz + off, m * 8, cudaMemcpyHostToDevice, st));
-    const double* dd = nullptr;
-    rc = upload_drift(h, drift_pts, stride, off, m, &dd); if (rc) return rc;
-    CU(h, cudaEventRecord(h->ev[10], st));
-    rc = run_to_host(h, m, z_out + off, ss_out + off, [&](int64_t o, int64_t c, double* dz, double* dss) {
-        Src s{false, 0, 0, 0, dp, dp + m, dp + 2 * m, o, c, dd, m, o};
-        return run_solve(h, s, dz, dss);
-    });
-    if (rc) return rc;
-    h->tm[6] += ev_ms(h->ev[9], h->ev[10]);
-    h->tm[4] += ev_ms(h->ev[7], h->ev[8]);
-    return KB200_OK;
-}
-
-extern "C" int kb200_execute_points(kb200_handle h, int64_t m,
-                                    const double* px, const double* py, const double* pz,
-                                    const double* drift_pts, double* z_out, double* ss_out) {
-    if (!h) return KB200_EBADARG;
-    return exec_points_impl(h, 0, m, px, py, pz, drift_pts, m, z_out, ss_out);
-}
-
-// grid points [first, first + count); drift columns cover the caller's slice [cfirst, cfirst + ccount) and
-// z_out / ss_out are indexed relative to cfirst
-static int exec_grid_impl(kb200_ctx* h, int64_t nx, int64_t ny, int64_t nz,
-                          const double* gx, const double* gy, const double* gz,
-                          const double* drift_pts, int64_t cfirst, int64_t ccount, int64_t first, int64_t count,
-                          double* z_out, double* ss_out) {
-    int rc = check_ready(h); if (rc) return rc;
-    rc = check_grid(h, nx, ny, nz, first, count); if (rc) return rc;
-    if (count == 0) return KB200_OK;
-    if (!gx || !gy || (h->dim == 3 && !gz) || !z_out || !ss_out) return fail(h, KB200_EBADARG, "null pointer");
-    if (n_host_drift(h) && !drift_pts) return fail(h, KB200_EBADARG, "drift values at the points are required");
-    cudaStream_t st = h->stream;
-    CU(h, h->wAxes.reserve((size_t)(nx + ny + nz) * 8));
-    double* da = h->wAxes.as<double>();
-    CU(h, cudaEventRecord(h->ev[9], st));
-    CU(h, cudaMemcpyAsync(da, gx, nx * 8, cudaMemcpyHostToDevice, st));
-    CU(h, cudaMemcpyAsync(da + nx, gy, ny * 8, cudaMemcpyHostToDevice, st));
-    if (h->dim == 3) CU(h, cudaMemcpyAsync(da + nx + ny, gz, nz * 8, cudaMemcpyHostToDevice, st));
-    const double* dd = nullptr;
-    rc = upload_drift(h, drift_pts, ccount, first - cfirst, count, &dd); if (rc) return rc;
-    CU(h, cudaEventRecord(h->ev[10], st));
-    rc = run_to_host(h, count, z_out + (first - cfirst), ss_out + (first - cfirst),
-                     [&](int64_t o, int64_t c, double* dz, double* dss) {
-        Src s{true, nx, ny, nz, da, da + nx, da + nx + ny, first + o, c, dd, count, o};
-        return run_solve(h, s, dz, dss);
-    });
-    if (rc) return rc;
-    h->tm[6] += ev_ms(h->ev[9], h->ev[10]);
-    h->tm[4] += ev_ms(h->ev[7], h->ev[8]);
-    return KB200_OK;
-}
-
-extern "C" int kb200_execute_grid(kb200_handle h, int64_t nx, int64_t ny, int64_t nz,
-                                  const double* gx, const double* gy, const double* gz,
-                                  const double* drift_pts, int64_t first, int64_t count,
-                                  double* z_out, double* ss_out) {
-    if (!h) return KB200_EBADARG;
-    return exec_grid_impl(h, nx, ny, nz, gx, gy, gz, drift_pts, first, count, first, count, z_out, ss_out);
+    return solve_dev(h, Src{true, nx, ny, nz, d_gx, d_gy, d_gz, first, count, d_drift_pts, count, 0}, d_z, d_ss);
 }
 
 // ---- moving window ----------------------------------------------------------
@@ -961,25 +939,10 @@ extern "C" int kb200_set_problem_knn(kb200_handle h, int dim, int64_t n,
                       exact_values, eps, 0, 0, nullptr);
     if (rc != KB200_OK) return rc;
     cudaStream_t st = h->stream;
-    const int nn = h->n, np = h->n_pad;
-    CU(h, h->wRaw.reserve((size_t)4 * nn * sizeof(double)));
-    double* raw = h->wRaw.as<double>();
-    double *rx = raw, *ry = raw + nn, *rz = raw + 2 * (size_t)nn, *rv = raw + 3 * (size_t)nn;
-    char* blob = h->blob.as<char>();
-    double* ax = reinterpret_cast<double*>(blob + h->off_ax);
-    double* ay = reinterpret_cast<double*>(blob + h->off_ay);
-    double* az = reinterpret_cast<double*>(blob + h->off_az);
+    const int nn = h->n;
     int launches = 0;
-    CU(h, cudaEventRecord(h->ev[0], st));
-    CU(h, cudaMemcpyAsync(rx, h->hx.data(), nn * 8, cudaMemcpyHostToDevice, st));
-    CU(h, cudaMemcpyAsync(ry, h->hy.data(), nn * 8, cudaMemcpyHostToDevice, st));
-    CU(h, cudaMemcpyAsync(rz, h->hz.data(), nn * 8, cudaMemcpyHostToDevice, st));
-    CU(h, cudaMemcpyAsync(rv, h->hval.data(), nn * 8, cudaMemcpyHostToDevice, st));
-    CU(h, cudaMemsetAsync(ax, 0, (size_t)np * 8, st));
-    CU(h, cudaMemsetAsync(ay, 0, (size_t)np * 8, st));
-    CU(h, cudaMemsetAsync(az, 0, (size_t)np * 8, st));
-    CU(h, kbk_adjust_data(h->dim, h->an, nn, rx, ry, rz, ax, ay, az, st)); ++launches;
-    CU(h, cudaEventRecord(h->ev[1], st));
+    rc = upload_data(h, false, &launches); if (rc) return rc;
+    const BlobView b = blob_view(h);
     // uniform cell grid with ~2 points per cell over the adjusted bounding box
     KnnParams& kp = h->kp;
     kp = KnnParams{};
@@ -1015,8 +978,8 @@ extern "C" int kb200_set_problem_knn(kb200_handle h, int dim, int64_t n,
     int* cell_of = sorig + nn;
     int* cell_start = h->kCells.as<int>();
     int* cursor = cell_start + (ncells + 1);
-    CU(h, kbk_knn_build(h->dim, nn, ax, ay, az, rv, kp, sx, sy, sz, sv, sorig, cell_of, cell_start, cursor,
-                        ncells, st, &launches));
+    CU(h, kbk_knn_build(h->dim, nn, b.ax, b.ay, b.az, raw_col(h, RAW_V), kp, sx, sy, sz, sv, sorig, cell_of, cell_start,
+                        cursor, ncells, st, &launches));
     if (h->nf) {                                   // value fields, field-major in the cell-sorted order
         const size_t fb = (size_t)h->nf * nn * sizeof(double);
         CU(h, h->kFields.reserve(2 * fb));
@@ -1025,17 +988,15 @@ extern "C" int kb200_set_problem_knn(kb200_handle h, int dim, int64_t n,
         CU(h, kbk_knn_sort_fields(nn, h->nf, sorig, raw_f, h->kFields.as<double>(), st)); ++launches;
         kp.values = h->kFields.as<double>(); kp.nv = h->nf;
     }
-    CU(h, cudaEventRecord(h->ev[2], st));
+    CU(h, cudaEventRecord(h->ev[EV_KNN_BUILT], st));
     CU(h, cudaStreamSynchronize(st));
-    h->tm[6] += ev_ms(h->ev[0], h->ev[1]);
-    h->tm[8] += ev_ms(h->ev[1], h->ev[2]);
+    h->tm[TM_H2D] += ev_ms(h->ev[EV_UPLOAD], h->ev[EV_ADJUSTED]);
+    h->tm[TM_KNN_SEARCH] += ev_ms(h->ev[EV_ADJUSTED], h->ev[EV_KNN_BUILT]);
     h->launches += launches;
     h->knn_ready = true;
     return KB200_OK;
 }
 
-
-// ---- moving window: execute ---------------------------------------------------------------------------------
 static int run_knn(kb200_ctx* h, int k, const Src& s, double* d_z, double* d_ss, int chol, int loo) {
     cudaStream_t st = h->stream;
     KnnParams kp = h->kp;
@@ -1048,11 +1009,7 @@ static int run_knn(kb200_ctx* h, int k, const Src& s, double* d_z, double* d_ss,
         double R = live >= 3 ? std::cbrt(cells * 3.0 / (4.0 * 3.14159265358979)) : (live == 2 ? std::sqrt(cells / 3.14159265358979) : 0.5 * cells);
         kp.r0 = (int)std::min(64.0, std::max(1.0, std::ceil(R)));
     }
-    PointSource ps{};
-    ps.grid = s.grid ? 1 : 0;
-    ps.px = s.a; ps.py = s.b; ps.pz = s.c; ps.gx = s.a; ps.gy = s.b; ps.gz = s.c;
-    ps.nx = s.nx; ps.ny = s.ny; ps.nz = s.nz; ps.first = s.first;
-    kp.ps = ps; kp.m = s.count; kp.z_out = d_z; kp.ss_out = d_ss; kp.flag = h->wFlag.as<int>(); kp.zstride = h->zstride;
+    kp.ps = s.point_source(); kp.m = s.count; kp.z_out = d_z; kp.ss_out = d_ss; kp.flag = h->wFlag.as<int>(); kp.zstride = h->zstride;
     CU(h, kbk_knn_solve(kp, chol, st, loo));
     h->launches += 1; h->solve_launches += 1;
     return KB200_OK;
@@ -1068,25 +1025,32 @@ static int check_knn(kb200_ctx* h, int k) {
     return KB200_OK;
 }
 
-// Run the moving window to HOST buffers and handle the solver flag: 2 = a local covariance block was not positive
-// definite (variogram not valid in this dimension) -> repeat with the pivoted-LU solver (dgesv semantics);
-// 1 = exactly singular local system -> ValueError('Singular matrix') (cok.pyx:176-179).
-template <class MakeSrc>
-static int knn_to_host(kb200_ctx* h, int k, int64_t total, double* z_out, double* ss_out, MakeSrc make_src, int loo = 0) {
+// Run the moving window and handle the solver flag: 2 = a local covariance block was not positive definite (variogram
+// not valid in this dimension) -> repeat with the pivoted-LU solver (dgesv semantics); 1 = exactly singular local
+// system -> ValueError('Singular matrix') (cok.pyx:176-179). run(chol) enqueues the whole call between EV_RUN and
+// EV_RUN_END.
+template <class Run>
+static int knn_retry(kb200_ctx* h, Run run) {
     int* flag = h->wFlag.as<int>();
     for (int chol = 1; chol >= 0; --chol) {
         CU(h, cudaMemsetAsync(flag, 0, sizeof(int), h->stream));
-        int rc = run_to_host(h, total, z_out, ss_out, [&](int64_t o, int64_t c, double* dz, double* dss) {
-            return run_knn(h, k, make_src(o, c), dz, dss, chol, loo);
-        });
-        if (rc) return rc;
+        int rc = run(chol); if (rc) return rc;
         int hflag = 0;
-        CU(h, cudaMemcpy(&hflag, flag, sizeof(int), cudaMemcpyDeviceToHost));
-        h->tm[9] += ev_ms(h->ev[7], h->ev[8]);
+        CU(h, cudaMemcpyAsync(&hflag, flag, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+        CU(h, cudaStreamSynchronize(h->stream));
+        h->tm[TM_KNN_SOLVE] += ev_ms(h->ev[EV_RUN], h->ev[EV_RUN_END]);
         if (hflag == 0) return KB200_OK;
         if (hflag != 2 || chol == 0) return fail(h, KB200_ESINGULAR, "Singular matrix");
     }
     return KB200_OK;
+}
+
+static int knn_to_host(kb200_ctx* h, int k, const Src& s, double* z_out, double* ss_out, int loo) {
+    return knn_retry(h, [&](int chol) {
+        return run_to_host(h, s.count, z_out, ss_out, [&](int64_t o, int64_t c, double* dz, double* dss) {
+            return run_knn(h, k, s.sub(o, c), dz, dss, chol, loo);
+        });
+    });
 }
 
 extern "C" int kb200_execute_knn_grid_dev(kb200_handle h, int k, int64_t nx, int64_t ny, int64_t nz,
@@ -1095,81 +1059,101 @@ extern "C" int kb200_execute_knn_grid_dev(kb200_handle h, int k, int64_t nx, int
     int rc = check_knn(h, k); if (rc) return rc;
     rc = check_grid(h, nx, ny, nz, first, count); if (rc) return rc;
     if (count == 0) return KB200_OK;
-    if (!d_gx || !d_gy || (h->dim == 3 && !d_gz) || !d_z || !d_ss) return fail(h, KB200_EBADARG, "null pointer");
-    Src s{true, nx, ny, nz, d_gx, d_gy, d_gz, first, count, nullptr, 0, 0};
+    rc = check_io(h, d_gx, d_gy, d_gz, nullptr, d_z, d_ss); if (rc) return rc;
+    const Src s{true, nx, ny, nz, d_gx, d_gy, d_gz, first, count, nullptr, 0, 0};
     h->zstride = count;
-    int* flag = h->wFlag.as<int>();
-    for (int chol = 1; chol >= 0; --chol) {
-        CU(h, cudaMemsetAsync(flag, 0, sizeof(int), h->stream));
-        CU(h, cudaEventRecord(h->ev[7], h->stream));
-        rc = run_knn(h, k, s, d_z, d_ss, chol); if (rc) return rc;
-        CU(h, cudaEventRecord(h->ev[8], h->stream));
-        int hflag = 0;
-        CU(h, cudaMemcpyAsync(&hflag, flag, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-        CU(h, cudaStreamSynchronize(h->stream));
-        h->tm[9] += ev_ms(h->ev[7], h->ev[8]);
-        if (hflag == 0) return KB200_OK;
-        if (hflag != 2 || chol == 0) return fail(h, KB200_ESINGULAR, "Singular matrix");
-    }
+    return knn_retry(h, [&](int chol) {
+        CU(h, cudaEventRecord(h->ev[EV_RUN], h->stream));
+        int rc = run_knn(h, k, s, d_z, d_ss, chol, 0); if (rc) return rc;
+        CU(h, cudaEventRecord(h->ev[EV_RUN_END], h->stream));
+        return KB200_OK;
+    });
+}
+
+// ---- execute to host buffers ----------------------------------------------------------------------------------
+// The prediction points of a host execute call: explicit points or grid axes. The caller's arrays (its outputs and
+// host drift columns) cover its slice [cfirst, cfirst + ccount) of the points; this call computes [first, first + count).
+struct Query {
+    bool grid; int64_t nx, ny, nz;
+    const double *a, *b, *c;      // px, py, pz or gx, gy, gz
+    const double* drift;
+    int64_t cfirst, ccount, first, count;
+};
+
+// host drift columns [n_host][stride] -> device columns [n_host][m] holding items [off, off + m) of each column
+static int upload_drift(kb200_ctx* h, const double* drift_pts, int64_t stride, int64_t off, int64_t m, const double** dd) {
+    *dd = nullptr;
+    const int nh = n_host_drift(h);
+    if (!nh) return KB200_OK;
+    CU(h, h->wDrift.reserve((size_t)nh * m * 8));
+    for (int c = 0; c < nh; ++c)
+        CU(h, cudaMemcpyAsync(h->wDrift.as<double>() + (size_t)c * m, drift_pts + (size_t)c * stride + off, (size_t)m * 8,
+                              cudaMemcpyHostToDevice, h->stream));
+    *dd = h->wDrift.as<double>();
     return KB200_OK;
 }
 
-static int exec_knn_grid_impl(kb200_ctx* h, int k, int64_t nx, int64_t ny, int64_t nz,
-                              const double* gx, const double* gy, const double* gz,
-                              int64_t cfirst, int64_t first, int64_t count, double* z_out, double* ss_out) {
-    int rc = check_knn(h, k); if (rc) return rc;
-    rc = check_grid(h, nx, ny, nz, first, count); if (rc) return rc;
-    if (count == 0) return KB200_OK;
-    if (!gx || !gy || (h->dim == 3 && !gz) || !z_out || !ss_out) return fail(h, KB200_EBADARG, "null pointer");
+// The query's explicit points [first, first + count) (or all its grid axes) and its host drift columns to the device,
+// timed as h2d (EV_H2D .. EV_H2D_END). *s is the device source of the query's points; s->sub(o, c) that of [o, o + c).
+static int upload_query(kb200_ctx* h, const Query& q, Src* s) {
     cudaStream_t st = h->stream;
-    CU(h, h->wAxes.reserve((size_t)(nx + ny + nz) * 8));
-    double* da = h->wAxes.as<double>();
-    CU(h, cudaEventRecord(h->ev[9], st));
-    CU(h, cudaMemcpyAsync(da, gx, nx * 8, cudaMemcpyHostToDevice, st));
-    CU(h, cudaMemcpyAsync(da + nx, gy, ny * 8, cudaMemcpyHostToDevice, st));
-    if (h->dim == 3) CU(h, cudaMemcpyAsync(da + nx + ny, gz, nz * 8, cudaMemcpyHostToDevice, st));
-    CU(h, cudaEventRecord(h->ev[10], st));
-    rc = knn_to_host(h, k, count, z_out + (first - cfirst), ss_out + (first - cfirst), [&](int64_t o, int64_t c) {
-        return Src{true, nx, ny, nz, da, da + nx, da + nx + ny, first + o, c, nullptr, 0, 0};
-    });
-    if (rc) return rc;
-    h->tm[6] += ev_ms(h->ev[9], h->ev[10]);
+    const int64_t off = q.first - q.cfirst;
+    const int64_t len[3] = {q.grid ? q.nx : q.count, q.grid ? q.ny : q.count, q.grid ? q.nz : q.count};
+    const double* src[3] = {q.a, q.b, q.c};
+    CU(h, h->wPts.reserve((size_t)(len[0] + len[1] + len[2]) * 8));
+    double* col[3] = {h->wPts.as<double>(), h->wPts.as<double>() + len[0], h->wPts.as<double>() + len[0] + len[1]};
+    CU(h, cudaEventRecord(h->ev[EV_H2D], st));
+    for (int r = 0; r < (h->dim == 3 ? 3 : 2); ++r)
+        CU(h, cudaMemcpyAsync(col[r], src[r] + (q.grid ? 0 : off), len[r] * 8, cudaMemcpyHostToDevice, st));
+    const double* dd = nullptr;
+    int rc = upload_drift(h, q.drift, q.ccount, off, q.count, &dd); if (rc) return rc;
+    CU(h, cudaEventRecord(h->ev[EV_H2D_END], st));
+    *s = Src{q.grid, q.nx, q.ny, q.nz, col[0], col[1], col[2], q.grid ? q.first : 0, q.count, dd, q.count, 0};
     return KB200_OK;
+}
+
+// One handle's share of a host execute call, by the global solve or (knn) the moving window with k neighbours
+static int exec_host(kb200_ctx* h, bool knn, int k, const Query& q, double* z_out, double* ss_out) {
+    int rc = knn ? check_knn(h, k) : check_ready(h); if (rc) return rc;
+    if (q.grid) { rc = check_grid(h, q.nx, q.ny, q.nz, q.first, q.count); if (rc) return rc; }
+    if (q.count <= 0) return KB200_OK;
+    rc = check_io(h, q.a, q.b, q.c, q.drift, z_out, ss_out); if (rc) return rc;
+    Src s{};
+    rc = upload_query(h, q, &s); if (rc) return rc;
+    const int64_t off = q.first - q.cfirst;
+    rc = knn ? knn_to_host(h, k, s, z_out + off, ss_out + off, 0)
+             : run_to_host(h, q.count, z_out + off, ss_out + off, [&](int64_t o, int64_t c, double* dz, double* dss) {
+                   return run_solve(h, s.sub(o, c), dz, dss);
+               });
+    if (rc) return rc;
+    h->tm[TM_H2D] += ev_ms(h->ev[EV_H2D], h->ev[EV_H2D_END]);
+    if (!knn) h->tm[TM_SOLVE] += ev_ms(h->ev[EV_RUN], h->ev[EV_RUN_END]);
+    return KB200_OK;
+}
+
+extern "C" int kb200_execute_points(kb200_handle h, int64_t m,
+                                    const double* px, const double* py, const double* pz,
+                                    const double* drift_pts, double* z_out, double* ss_out) {
+    return exec_host(h, false, 0, Query{false, 0, 0, 0, px, py, pz, drift_pts, 0, m, 0, m}, z_out, ss_out);
+}
+
+extern "C" int kb200_execute_grid(kb200_handle h, int64_t nx, int64_t ny, int64_t nz,
+                                  const double* gx, const double* gy, const double* gz,
+                                  const double* drift_pts, int64_t first, int64_t count,
+                                  double* z_out, double* ss_out) {
+    return exec_host(h, false, 0, Query{true, nx, ny, nz, gx, gy, gz, drift_pts, first, count, first, count}, z_out, ss_out);
 }
 
 extern "C" int kb200_execute_knn_grid(kb200_handle h, int k, int64_t nx, int64_t ny, int64_t nz,
                                       const double* gx, const double* gy, const double* gz,
                                       int64_t first, int64_t count, double* z_out, double* ss_out) {
-    if (!h) return KB200_EBADARG;
-    return exec_knn_grid_impl(h, k, nx, ny, nz, gx, gy, gz, first, first, count, z_out, ss_out);
-}
-
-static int exec_knn_points_impl(kb200_ctx* h, int k, int64_t off, int64_t m,
-                                const double* px, const double* py, const double* pz, double* z_out, double* ss_out) {
-    int rc = check_knn(h, k); if (rc) return rc;
-    if (m <= 0) return KB200_OK;
-    if (!px || !py || (h->dim == 3 && !pz) || !z_out || !ss_out) return fail(h, KB200_EBADARG, "null pointer");
-    cudaStream_t st = h->stream;
-    CU(h, h->wPts.reserve((size_t)3 * m * 8));
-    double* dp = h->wPts.as<double>();
-    CU(h, cudaEventRecord(h->ev[9], st));
-    CU(h, cudaMemcpyAsync(dp, px + off, m * 8, cudaMemcpyHostToDevice, st));
-    CU(h, cudaMemcpyAsync(dp + m, py + off, m * 8, cudaMemcpyHostToDevice, st));
-    if (h->dim == 3) CU(h, cudaMemcpyAsync(dp + 2 * m, pz + off, m * 8, cudaMemcpyHostToDevice, st));
-    CU(h, cudaEventRecord(h->ev[10], st));
-    rc = knn_to_host(h, k, m, z_out + off, ss_out + off, [&](int64_t o, int64_t c) {
-        return Src{false, 0, 0, 0, dp, dp + m, dp + 2 * m, o, c, nullptr, 0, 0};
-    });
-    if (rc) return rc;
-    h->tm[6] += ev_ms(h->ev[9], h->ev[10]);
-    return KB200_OK;
+    return exec_host(h, true, k, Query{true, nx, ny, nz, gx, gy, gz, nullptr, first, count, first, count}, z_out, ss_out);
 }
 
 extern "C" int kb200_execute_knn_points(kb200_handle h, int k, int64_t m,
                                         const double* px, const double* py, const double* pz,
                                         double* z_out, double* ss_out) {
-    if (!h) return KB200_EBADARG;
-    return exec_knn_points_impl(h, k, 0, m, px, py, pz, z_out, ss_out);
+    return exec_host(h, true, k, Query{false, 0, 0, 0, px, py, pz, nullptr, 0, m, 0, m}, z_out, ss_out);
 }
 
 // ---- single-process multi-GPU: a group of handles driven by one caller thread --------------------------------
@@ -1200,10 +1184,14 @@ static int group_parallel(kb200_group_ctx* g, F f) {
     return KB200_OK;
 }
 
-static void shard_block(int64_t count, int rank, int world, int64_t* first, int64_t* n) {
-    const int64_t base = count / world, rem = count % world;
-    *first = rank * base + std::min<int64_t>(rank, rem);
-    *n = base + (rank < rem ? 1 : 0);
+// f(member, first, n) on every member, with points [0, count) cut into one contiguous block per member
+template <class F>
+static int group_sharded(kb200_group_ctx* g, int64_t count, F f) {
+    if (!g || g->m.empty()) return KB200_EBADARG;
+    const int64_t G = (int64_t)g->m.size(), base = count / G, rem = count % G;
+    return group_parallel(g, [&](int i) {
+        return f(g->m[i], i * base + std::min<int64_t>(i, rem), base + (i < rem ? 1 : 0));
+    });
 }
 
 extern "C" int kb200_group_create(kb200_group* out, int n_gpus, const int* devices) {
@@ -1291,48 +1279,35 @@ extern "C" int kb200_group_execute_grid(kb200_group g, int64_t nx, int64_t ny, i
                                         const double* gx, const double* gy, const double* gz,
                                         const double* drift_pts, int64_t first, int64_t count,
                                         double* z_out, double* ss_out) {
-    if (!g || g->m.empty()) return KB200_EBADARG;
-    const int G = (int)g->m.size();
-    return group_parallel(g, [&](int i) {
-        int64_t f, c; shard_block(count, i, G, &f, &c);
-        return exec_grid_impl(g->m[i], nx, ny, nz, gx, gy, gz, drift_pts, first, count, first + f, c, z_out, ss_out);
+    return group_sharded(g, count, [&](kb200_ctx* h, int64_t f, int64_t c) {
+        return exec_host(h, false, 0, Query{true, nx, ny, nz, gx, gy, gz, drift_pts, first, count, first + f, c}, z_out, ss_out);
     });
 }
 
 extern "C" int kb200_group_execute_points(kb200_group g, int64_t m,
                                           const double* px, const double* py, const double* pz,
                                           const double* drift_pts, double* z_out, double* ss_out) {
-    if (!g || g->m.empty()) return KB200_EBADARG;
-    const int G = (int)g->m.size();
-    return group_parallel(g, [&](int i) {
-        int64_t f, c; shard_block(m, i, G, &f, &c);
-        return exec_points_impl(g->m[i], f, c, px, py, pz, drift_pts, m, z_out, ss_out);
+    return group_sharded(g, m, [&](kb200_ctx* h, int64_t f, int64_t c) {
+        return exec_host(h, false, 0, Query{false, 0, 0, 0, px, py, pz, drift_pts, 0, m, f, c}, z_out, ss_out);
     });
 }
 
 extern "C" int kb200_group_execute_knn_grid(kb200_group g, int k, int64_t nx, int64_t ny, int64_t nz,
                                             const double* gx, const double* gy, const double* gz,
                                             int64_t first, int64_t count, double* z_out, double* ss_out) {
-    if (!g || g->m.empty()) return KB200_EBADARG;
-    const int G = (int)g->m.size();
-    return group_parallel(g, [&](int i) {
-        int64_t f, c; shard_block(count, i, G, &f, &c);
-        return exec_knn_grid_impl(g->m[i], k, nx, ny, nz, gx, gy, gz, first, first + f, c, z_out, ss_out);
+    return group_sharded(g, count, [&](kb200_ctx* h, int64_t f, int64_t c) {
+        return exec_host(h, true, k, Query{true, nx, ny, nz, gx, gy, gz, nullptr, first, count, first + f, c}, z_out, ss_out);
     });
 }
 
 extern "C" int kb200_group_execute_knn_points(kb200_group g, int k, int64_t m,
                                               const double* px, const double* py, const double* pz,
                                               double* z_out, double* ss_out) {
-    if (!g || g->m.empty()) return KB200_EBADARG;
-    const int G = (int)g->m.size();
-    return group_parallel(g, [&](int i) {
-        int64_t f, c; shard_block(m, i, G, &f, &c);
-        return exec_knn_points_impl(g->m[i], k, f, c, px, py, pz, z_out, ss_out);
+    return group_sharded(g, m, [&](kb200_ctx* h, int64_t f, int64_t c) {
+        return exec_host(h, true, k, Query{false, 0, 0, 0, px, py, pz, nullptr, 0, m, f, c}, z_out, ss_out);
     });
 }
 
-// ---- debug taps (tests only) ------------------------------------------------
 // ---- constructor-side helpers (SURVEY.md 8f next-2) -----------------------------------------------
 extern "C" int kb200_experimental_variogram(kb200_handle h, int dim, int64_t n,
                                             const double* x, const double* y, const double* z, const double* values,
@@ -1394,22 +1369,19 @@ extern "C" int kb200_statistics(kb200_handle h, double* delta, double* sigma) {
                            "not to kb200_set_values fields");
     if (h->gform) return fail(h, KB200_EUNSUPPORTED, "cross-validation statistics need the positive definite "
                               "covariance form (this problem runs on the general fallback)");
-    if (!h->factor_live) return fail(h, KB200_ESTATE, "the Cholesky factor is not on this handle "
-                                     "(problem received through kb200_blob_commit)");
+    if (!h->local_factor) return fail(h, KB200_ESTATE, "the Cholesky factor is not on this handle "
+                                      "(problem received through kb200_blob_commit)");
     cudaSetDevice(h->device);
     cudaStream_t st = h->stream;
     const int nn = h->n, np = h->n_pad;
-    char* blob = h->blob.as<char>();
-    const double* ax = reinterpret_cast<double*>(blob + h->off_ax);
-    const double* ay = reinterpret_cast<double*>(blob + h->off_ay);
-    const double* az = reinterpret_cast<double*>(blob + h->off_az);
-    const double* Hz = h->wF.as<double>() + (size_t)h->aux_cols * np;
+    const BlobView b = blob_view(h);
+    const double* Hz = aux_block(h, AUX_H);
     const int K = h->n_rl + h->n_hd;                       // Hz row K = L^-1 1, row K+1 = L^-1 Z
     CU(h, h->wVario.reserve((size_t)nn * (2 * sizeof(double) + sizeof(int)) + 256));
     double* d_delta = h->wVario.as<double>();
     double* d_sigma = d_delta + nn;
     int* d_dup = reinterpret_cast<int*>(d_sigma + nn);
-    CU(h, kbk_statistics(h->dim, nn, ax, ay, az, h->wC.as<double>(), h->ld,
+    CU(h, kbk_statistics(h->dim, nn, b.ax, b.ay, b.az, h->wC.as<double>(), h->ld,
                          Hz + (size_t)K * np, Hz + (size_t)(K + 1) * np, d_dup, d_delta, d_sigma, st));
     CU(h, cudaMemcpyAsync(delta, d_delta, (size_t)nn * 8, cudaMemcpyDeviceToHost, st));
     CU(h, cudaMemcpyAsync(sigma, d_sigma, (size_t)nn * 8, cudaMemcpyDeviceToHost, st));
@@ -1418,6 +1390,7 @@ extern "C" int kb200_statistics(kb200_handle h, double* delta, double* sigma) {
     return KB200_OK;
 }
 
+// ---- debug tap (tests only) ------------------------------------------------
 extern "C" int64_t kb200_debug_fetch(kb200_handle h, int what, double* out, int64_t cap) {
     if (!h || !out) return KB200_EBADARG;
     if (!h->described) return KB200_ESTATE;
@@ -1432,10 +1405,8 @@ extern "C" int64_t kb200_debug_fetch(kb200_handle h, int what, double* out, int6
         size_t nc = (size_t)h->K1 * h->na;            // Sinv ((K+1)^2) | phi_v ((K+1) per field)
         size_t total = nU + nc + 1;
         if ((int64_t)total > cap) return KB200_EBADARG;
-        const double* Uz = h->wF.as<double>() + (size_t)2 * h->aux_cols * h->n_pad;
-        if (cudaMemcpy(out, Uz, nU * 8, cudaMemcpyDeviceToHost) != cudaSuccess) return KB200_ECUDA;
-        if (cudaMemcpy(out + nU, h->blob.as<char>() + h->off_consts, nc * 8,
-                       cudaMemcpyDeviceToHost) != cudaSuccess) return KB200_ECUDA;
+        if (cudaMemcpy(out, aux_block(h, AUX_U), nU * 8, cudaMemcpyDeviceToHost) != cudaSuccess) return KB200_ECUDA;
+        if (cudaMemcpy(out + nU, blob_view(h).consts, nc * 8, cudaMemcpyDeviceToHost) != cudaSuccess) return KB200_ECUDA;
         out[total - 1] = h->vg.c0;
         return (int64_t)total;
     } else return KB200_EBADARG;
@@ -1455,8 +1426,8 @@ extern "C" int kb200_loo(kb200_handle h, double* z_out, double* ss_out) {
     if (!h->ready) return fail(h, KB200_ESTATE, "no factored problem: call kb200_set_problem first");
     if (h->gform == 2) return fail(h, KB200_EUNSUPPORTED, "leave-one-out needs the inverse of the kriging matrix; "
                                    "the pseudo-inverse (pseudo_inv=True) does not give it");
-    if (!h->inv_live) return fail(h, KB200_ESTATE, "the factorisation is not on this handle "
-                                  "(problem received through kb200_blob_commit)");
+    if (!h->local_factor) return fail(h, KB200_ESTATE, "the factorisation is not on this handle "
+                                      "(problem received through kb200_blob_commit)");
     cudaSetDevice(h->device);
     cudaStream_t st = h->stream;
     const int nn = h->n, np = h->n_pad, nv = h->nf ? h->nf : 1;
@@ -1473,18 +1444,14 @@ extern "C" int kb200_loo(kb200_handle h, double* z_out, double* ss_out) {
     int* off = cnt + nn;
     int* slist = off + nn + 1;
     int* bad = slist + nn;
-    char* blob = h->blob.as<char>();
-    const double* ax = reinterpret_cast<double*>(blob + h->off_ax);
-    const double* ay = reinterpret_cast<double*>(blob + h->off_ay);
-    const double* az = reinterpret_cast<double*>(blob + h->off_az);
-    const double* raw = h->wRaw.as<double>();
+    const BlobView b = blob_view(h);
     int launches = 0;
 
     // exact_values: stations within eps of each other (counts, then the lists at host-scanned offsets)
     std::vector<int> hcnt, hoff, hst;
     int* pj = nullptr; double* pd = nullptr;
     if (h->vg.exact) {
-        CU(h, kbk_loo_pairs(h->dim, nn, ax, ay, az, h->vg.eps, cnt, nullptr, nullptr, nullptr, st)); ++launches;
+        CU(h, kbk_loo_pairs(h->dim, nn, b.ax, b.ay, b.az, h->vg.eps, cnt, nullptr, nullptr, nullptr, st)); ++launches;
         hcnt.resize(nn);
         CU(h, cudaMemcpyAsync(hcnt.data(), cnt, (size_t)nn * sizeof(int), cudaMemcpyDeviceToHost, st));
         CU(h, cudaStreamSynchronize(st));
@@ -1503,7 +1470,7 @@ extern "C" int kb200_loo(kb200_handle h, double* z_out, double* ss_out) {
             pj = reinterpret_cast<int*>(pd + tot);
             CU(h, cudaMemcpyAsync(off, hoff.data(), (size_t)(nn + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
             CU(h, cudaMemcpyAsync(slist, hst.data(), hst.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-            CU(h, kbk_loo_pairs(h->dim, nn, ax, ay, az, h->vg.eps, cnt, off, pj, pd, st)); ++launches;
+            CU(h, kbk_loo_pairs(h->dim, nn, b.ax, b.ay, b.az, h->vg.eps, cnt, off, pj, pd, st)); ++launches;
         }
     }
 
@@ -1511,23 +1478,23 @@ extern "C" int kb200_loo(kb200_handle h, double* z_out, double* ss_out) {
     p.n = nn; p.n_pad = np; p.ld = h->ld; p.K1 = h->K1; p.nv = nv; p.gform = h->gform; p.nchunks = nch;
     p.tol = KB_LOO_TOL; p.vg = h->vg;
     p.W = h->wW.as<double>(); p.G = h->wC.as<double>(); p.part = part;
-    p.Uz = h->wF.as<double>() + (size_t)2 * h->aux_cols * np;
-    p.consts = reinterpret_cast<const double*>(blob + h->off_consts);
-    p.Z = h->nf ? raw + (size_t)(4 + h->n_hd) * nn : raw + 3 * (size_t)nn;      // wRaw: x | y | z | v | drift | fields
+    p.Uz = aux_block(h, AUX_U);
+    p.consts = b.consts;
+    p.Z = kriged_values(h);
     p.pii = pii; p.alpha = alpha; p.z_out = dz; p.ss_out = dss; p.bad = bad;
     const int big = INT_MAX;
     CU(h, cudaMemcpyAsync(bad, &big, sizeof(int), cudaMemcpyHostToDevice, st));
-    CU(h, cudaEventRecord(h->ev[7], st));
+    CU(h, cudaEventRecord(h->ev[EV_RUN], st));
     if (h->gform == 0) { CU(h, kbk_loo_colsq(p.W, p.ld, nn, part, st)); ++launches; }
     CU(h, kbk_loo_finalize(p, st)); ++launches;
     if (!hst.empty()) { CU(h, kbk_loo_dup(p, (int)hst.size(), slist, off, pj, pd, st)); ++launches; }
-    CU(h, cudaEventRecord(h->ev[8], st));
+    CU(h, cudaEventRecord(h->ev[EV_RUN_END], st));
     int hbad = big;
     CU(h, cudaMemcpyAsync(&hbad, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
     CU(h, cudaMemcpyAsync(z_out, dz, (size_t)nv * nn * sizeof(double), cudaMemcpyDeviceToHost, st));
     CU(h, cudaMemcpyAsync(ss_out, dss, (size_t)nn * sizeof(double), cudaMemcpyDeviceToHost, st));
     CU(h, cudaStreamSynchronize(st));
-    h->tm[4] += ev_ms(h->ev[7], h->ev[8]);
+    h->tm[TM_SOLVE] += ev_ms(h->ev[EV_RUN], h->ev[EV_RUN_END]);
     h->launches += launches; h->solve_launches += launches;
     if (hbad != big)
         return fail(h, KB200_ESINGULAR, "leave-one-out: without station " + std::to_string(hbad) +
@@ -1539,9 +1506,7 @@ extern "C" int kb200_knn_loo(kb200_handle h, int k, double* z_out, double* ss_ou
     int rc = check_knn(h, k); if (rc) return rc;
     if (k > h->n - 1) return fail(h, KB200_EBADARG, "leave-one-out: n_closest_points must be at most n - 1");
     if (!z_out || !ss_out) return fail(h, KB200_EBADARG, "null pointer");
-    const int nn = h->n;
-    const double* raw = h->wRaw.as<double>();      // the stations' raw coordinates are the query points
-    return knn_to_host(h, k, nn, z_out, ss_out, [&](int64_t o, int64_t c) {
-        return Src{false, 0, 0, 0, raw, raw + nn, raw + 2 * (size_t)nn, o, c, nullptr, 0, 0};
-    }, 1);
+    // the stations' raw coordinates are the query points
+    const Src s{false, 0, 0, 0, raw_col(h, RAW_X), raw_col(h, RAW_Y), raw_col(h, RAW_Z), 0, h->n, nullptr, 0, 0};
+    return knn_to_host(h, k, s, z_out, ss_out, 1);
 }
