@@ -566,9 +566,7 @@ static int factor_general(kb200_ctx* h, const BlobView& b, double c0, float* t_c
     CU(h, cudaEventRecord(h->ev[EV_FACTOR], st));
     CU(h, kbk_assemble(h->dim, h->vg, nn, np, ld, b.ax, b.ay, b.az, G, st)); ++*launches;
     CU(h, h->wVario.reserve(kbk_general_inverse_workspace_bytes(np)));
-    const char* gj_env = std::getenv("KB200_GJ");            // "scalar": the tests' cross-check of the blocked default
-    CU(h, kbk_general_inverse(G, ld, nn, np, h->wVario.p, flag, 3.6e-15 * h->vg.c0, st, launches,
-                              gj_env && gj_env[0] == 's'));
+    CU(h, kbk_general_inverse(G, ld, np, h->wVario.p, flag, 3.6e-15 * h->vg.c0, st, launches));
     CU(h, cudaEventRecord(h->ev[EV_INVERT], st));
     int hflag = 0;
     CU(h, cudaMemcpyAsync(&hflag, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -612,7 +610,7 @@ static int factor_cholesky_pack(kb200_ctx* h, const BlobView& b, int* launches) 
         *launches += 2;                        // row scales + pack
         CU(h, cudaStreamSynchronize(st));      // toff is a host temporary
     } else {
-        CU(h, kbk_pack(h->dtype, W, ld, nn, np, h->na, Uz, h->pm, b.tiles, st)); ++*launches;
+        CU(h, kbk_pack(W, ld, nn, np, h->na, Uz, h->pm, b.tiles, st)); ++*launches;
     }
     return 0;
 }

@@ -225,9 +225,49 @@ __device__ __forceinline__ void kb_dmma_16x8x4(double* c, const double* a, doubl
 
 // W tile order of the fp64 solve kernel (KB_BM x KB_BK, element (r, k)):  [m16 tile r/16][k/4][lane (r%8)*4 + k%4][(r/8)%2]
 // = the m16n8k4 A fragment (rows g and g + 8) of each lane as one double2, so one LDS.128 over the 32 lanes reads 512
-// contiguous bytes (conflict-free); written by pack_kernel<double> / pack_gform_kernel (factor.cu). The RHS tile keeps
+// contiguous bytes (conflict-free); written by pack_kernel / pack_gform_kernel (factor.cu). The RHS tile keeps
 // the m8n8k4-era order ((k/4)*NT + n/8)*32 + (n%8)*4 + k%4, which already is the m16n8k4 B fragment: one LDS.64 over
 // 256 contiguous bytes.
+
+// ---- mbarrier + 1-D bulk copy (TMA engine, SASS UBLKCP): the toolkit of the pipelined kernels ----------------
+__device__ __forceinline__ uint32_t kb_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void kb_mbar_init(uint64_t* bar, int count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" :: "r"(kb_smem_u32(bar)), "r"(count));
+}
+// after the mbarrier inits of one thread, before the barrier that hands them to the block and the async proxy
+__device__ __forceinline__ void kb_fence_mbar_init() {
+    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
+}
+__device__ __forceinline__ void kb_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" :: "r"(kb_smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void kb_mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" :: "r"(kb_smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ bool kb_mbar_try_wait(uint64_t* bar, uint32_t parity) {
+    uint32_t ok;
+    asm volatile("{\n\t.reg .pred p;\n\t"
+                 "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+                 "selp.u32 %0, 1, 0, p;\n\t}\n"
+                 : "=r"(ok) : "r"(kb_smem_u32(bar)), "r"(parity) : "memory");
+    return ok != 0;
+}
+__device__ __forceinline__ void kb_mbar_wait(uint64_t* bar, uint32_t parity) {
+    // bounded spin: a lost transaction traps instead of hanging the GPU
+    for (uint32_t it = 0; it < (1u << 26); ++it)
+        if (kb_mbar_try_wait(bar, parity)) return;
+    __trap();
+}
+// generic-proxy global writes of this thread -> later read by the async proxy (bulk copies)
+__device__ __forceinline__ void kb_fence_publish_async() {
+    __threadfence();
+    asm volatile("fence.proxy.async.global;\n" ::: "memory");
+}
+__device__ __forceinline__ void kb_bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
+                 :: "r"(kb_smem_u32(dst)), "l"(src), "r"(bytes), "r"(kb_smem_u32(bar)) : "memory");
+}
 
 // ---- L2 cache policies for the bulk copies of the solve kernels ----------------------------------------------
 // The factor tile stream (W) is read by every CTA for every point tile: keep what L2 holds of it (evict_last; DESIGN.md §2
@@ -244,11 +284,10 @@ __device__ __forceinline__ uint64_t kb_policy_evict_first() {
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;\n" : "=l"(p));
     return p;
 }
-// 1-D bulk copy global -> shared through the TMA engine (SASS: UBLKCP) with an L2 cache policy
+// kb_bulk_g2s with an L2 cache policy
 __device__ __forceinline__ void kb_bulk_g2s_hint(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint64_t policy) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;\n"
-                 :: "r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src), "r"(bytes),
-                    "r"((uint32_t)__cvta_generic_to_shared(bar)), "l"(policy) : "memory");
+                 :: "r"(kb_smem_u32(dst)), "l"(src), "r"(bytes), "r"(kb_smem_u32(bar)), "l"(policy) : "memory");
 }
 
 // ---- warpgroup MMA (wgmma, sm_90a) helpers for the tensor-core solve kernels ---------------------------------

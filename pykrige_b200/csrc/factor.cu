@@ -586,69 +586,49 @@ __global__ void __launch_bounds__(256) dual_small_kernel(int n, int n_pad, int K
 }
 
 // ---------------------------------------------------------------------------
-// K2d  pack: tile (row block I, k tile kt) -> 4096 values in fragment order
-//   double (the fp64 DMMA solve kernel): element (r, k) of the tile lives at ((r/16)*4 + k/4)*64 + ((r%8)*4 + k%4)*2 +
-//   (r/8)%2, the m16n8k4 A-fragment order of common.cuh; float: ((k/4)*32 + r/8)*32 + (r%8)*4 + k%4
+// K2d  pack: tile (row block I, k tile kt) -> 4096 values in the fp64 solve kernel's order: element (r, k) of the tile
+//   lives at ((r/16)*4 + k/4)*64 + ((r%8)*4 + k%4)*2 + (r/8)%2, the m16n8k4 A-fragment order of common.cuh.
 // rows < n: W (lower triangle); rows [n, n+na): dual rows Uz^T; other rows 0.
-__device__ __forceinline__ void pack_rk(bool f64, int I, int kt, int e, int& r, int& k) {
-    if (f64) {       // e = ((m16 tile * 4 + k/4) * 32 + lane) * 2 + (r/8)%2, lane = (r%8)*4 + k%4
-        const int h = e & 1, lane = (e >> 1) & 31, k4 = (e >> 6) & 3, mt = e >> 8;
-        r = I * KB_BM + mt * 16 + 8 * h + (lane >> 2);
-        k = kt * KB_BK + k4 * 4 + (lane & 3);
-    } else {
-        const int lane = e & 31, mt = (e >> 5) & 31, k4 = e >> 10;
-        r = I * KB_BM + mt * 8 + (lane >> 2);
-        k = kt * KB_BK + k4 * 4 + (lane & 3);
-    }
+__device__ __forceinline__ void pack_rk(int I, int kt, int e, int& r, int& k) {
+    // e = ((m16 tile * 4 + k/4) * 32 + lane) * 2 + (r/8)%2, lane = (r%8)*4 + k%4
+    const int h = e & 1, lane = (e >> 1) & 31, k4 = (e >> 6) & 3, mt = e >> 8;
+    r = I * KB_BM + mt * 16 + 8 * h + (lane >> 2);
+    k = kt * KB_BK + k4 * 4 + (lane & 3);
 }
-template <typename T>
 __global__ void __launch_bounds__(256) pack_kernel(const double* __restrict__ W, int ld, int n, int n_pad, int na,
-                                                    const double* __restrict__ Uz, PackMap pm, T* __restrict__ out) {
+                                                    const double* __restrict__ Uz, PackMap pm, double* __restrict__ out) {
     int I = blockIdx.y, kt = blockIdx.x;
     if (kt >= pm.ktiles[I]) return;
-    T* o = out + ((size_t)pm.tile_off[I] + kt) * (KB_BM * KB_BK);
+    double* o = out + ((size_t)pm.tile_off[I] + kt) * (KB_BM * KB_BK);
     for (int e = threadIdx.x; e < KB_BM * KB_BK; e += 256) {
         int r, k;
-        pack_rk(sizeof(T) == sizeof(double), I, kt, e, r, k);
+        pack_rk(I, kt, e, r, k);
         double v = 0.0;
         if (r < n) { if (k <= r) v = W[(size_t)r * ld + k]; }
         else if (r < n + na) { if (k < n) v = Uz[(size_t)(r - n) * n_pad + k]; }
-        o[e] = (T)v;
+        o[e] = v;
     }
 }
 
 // ---------------------------------------------------------------------------
 // host-side launchers
-template <int DIM>
-static cudaError_t launch_assemble_dim(const VgParams& vg, int n, int n_pad, int ld,
-                                       const double* ax, const double* ay, const double* az, double* C,
-                                       cudaStream_t st) {
-    int nb = n_pad / 64;
-    int tiles = nb * (nb + 1) / 2;
-    switch (vg.model) {
-#define KB_CASE(M) case M: assemble_kernel<DIM, M><<<tiles, 256, 0, st>>>(vg, n, n_pad, ld, ax, ay, az, C); break;
-        KB_CASE(KB200_VG_LINEAR) KB_CASE(KB200_VG_POWER) KB_CASE(KB200_VG_GAUSSIAN)
-        KB_CASE(KB200_VG_EXPONENTIAL) KB_CASE(KB200_VG_SPHERICAL) KB_CASE(KB200_VG_HOLE_EFFECT) KB_CASE(KB200_VG_TABLE)
-#undef KB_CASE
-        default: return cudaErrorInvalidValue;
-    }
-    return cudaGetLastError();
-}
-
 cudaError_t kbk_adjust_data(int dim, const Aniso& an, int n, const double* x, const double* y, const double* z,
                             double* ax, double* ay, double* az, cudaStream_t st) {
-    int g = (n + 255) / 256;
-    if (dim == 2) adjust_data_kernel<2><<<g, 256, 0, st>>>(an, n, x, y, z, ax, ay, az);
-    else if (dim == 3) adjust_data_kernel<3><<<g, 256, 0, st>>>(an, n, x, y, z, ax, ay, az);
-    else adjust_data_kernel<KB_GEO><<<g, 256, 0, st>>>(an, n, x, y, z, ax, ay, az);
-    return cudaGetLastError();
+    return KbDims::dispatch(dim, [&](auto D) {
+        adjust_data_kernel<D><<<(n + 255) / 256, 256, 0, st>>>(an, n, x, y, z, ax, ay, az);
+        return cudaGetLastError();
+    });
 }
 
 cudaError_t kbk_assemble(int dim, const VgParams& vg, int n, int n_pad, int ld,
                          const double* ax, const double* ay, const double* az, double* C, cudaStream_t st) {
-    if (dim == 2) return launch_assemble_dim<2>(vg, n, n_pad, ld, ax, ay, az, C, st);
-    if (dim == 3) return launch_assemble_dim<3>(vg, n, n_pad, ld, ax, ay, az, C, st);
-    return launch_assemble_dim<KB_GEO>(vg, n, n_pad, ld, ax, ay, az, C, st);
+    const int nb = n_pad / 64;
+    return KbDims::dispatch(dim, [&](auto D) {
+        return KbModels::dispatch(vg.model, [&](auto M) {
+            assemble_kernel<D, M><<<nb * (nb + 1) / 2, 256, 0, st>>>(vg, n, n_pad, ld, ax, ay, az, C);
+            return cudaGetLastError();
+        });
+    });
 }
 
 cudaError_t kbk_factor_init() {
@@ -743,89 +723,19 @@ cudaError_t kbk_build_fz(int n, int n_pad, int n_rl, int n_hd, const double* ax,
     return cudaGetLastError();
 }
 
-cudaError_t kbk_pack(int dtype, const double* W, int ld, int n, int n_pad, int na, const double* Uz,
+cudaError_t kbk_pack(const double* W, int ld, int n, int n_pad, int na, const double* Uz,
                      const PackMap& pm, void* out, cudaStream_t st) {
-    int maxkt = 0;
-    for (int i = 0; i < pm.nrb; ++i) maxkt = pm.ktiles[i] > maxkt ? pm.ktiles[i] : maxkt;
-    dim3 grid(maxkt, pm.nrb);
-    if (dtype == KB200_F64) pack_kernel<double><<<grid, 256, 0, st>>>(W, ld, n, n_pad, na, Uz, pm, (double*)out);
-    else pack_kernel<float><<<grid, 256, 0, st>>>(W, ld, n, n_pad, na, Uz, pm, (float*)out);
+    pack_kernel<<<kb_pack_grid(pm), 256, 0, st>>>(W, ld, n, n_pad, na, Uz, pm, (double*)out);
     return cudaGetLastError();
 }
 
 // ---------------------------------------------------------------------------
 // General fallback when C is not positive definite (a variogram that is not conditionally negative
 // definite in the working dimension, e.g. hole-effect on dense 2-D scatter; the reference's LU still
-// inverts such systems, ok.py:663). In-place Gauss-Jordan inversion with partial pivoting, two
-// launches per column (memory-bound, O(n^3) traffic: a slow path for a corner case):
-//   gj_pivot : pivot search in column k, row swap, scale of the pivot row, capture of column k
-//   gj_update: a[i][j] -= col[i] * row[j] for i != k
-// followed by the column swaps in reverse order. The result G = C^-1 is then used in the
-// quadratic-form variant of the solve kernel (q = c^T G c through the lower triangle with doubled
+// inverts such systems, ok.py:663): in-place Gauss-Jordan inversion with partial pivoting, blocked by 64 columns
+// ("Blocked Gauss-Jordan" below), followed by the column swaps in reverse order. The result G = C^-1 is then used in
+// the quadratic-form variant of the solve kernel (q = c^T G c through the lower triangle with doubled
 // off-diagonals, DESIGN.md §3b).
-__global__ void __launch_bounds__(1024) gj_pivot_kernel(double* __restrict__ A, int ld, int n, int k,
-                                                         double* __restrict__ rowbuf, double* __restrict__ colbuf,
-                                                         int* __restrict__ piv, int* __restrict__ flag, double ptol) {
-    __shared__ double sval[1024];
-    __shared__ int sidx[1024];
-    const int tid = threadIdx.x;
-    double best = -1.0; int bi = k;
-    for (int i = k + tid; i < n; i += 1024) {
-        double v = fabs(A[(size_t)i * ld + k]);
-        if (v > best) { best = v; bi = i; }
-    }
-    sval[tid] = best; sidx[tid] = bi;
-    __syncthreads();
-    for (int o = 512; o > 0; o >>= 1) {
-        if (tid < o) {
-            if (sval[tid + o] > sval[tid] || (sval[tid + o] == sval[tid] && sidx[tid + o] < sidx[tid])) {
-                sval[tid] = sval[tid + o]; sidx[tid] = sidx[tid + o];
-            }
-        }
-        __syncthreads();
-    }
-    const int p = sidx[0];
-    if (tid == 0) { piv[k] = p; if (!(sval[0] > ptol) && *flag == 0) *flag = 1 + k; }   // ptol: rounding noise (this variant scales the pivot row, so redundant rows cancel to ~1 ulp, not 0)
-    if (p != k) {
-        for (int j = tid; j < n; j += 1024) {
-            double t = A[(size_t)k * ld + j]; A[(size_t)k * ld + j] = A[(size_t)p * ld + j]; A[(size_t)p * ld + j] = t;
-        }
-    }
-    __syncthreads();
-    double d = A[(size_t)k * ld + k];
-    if (!(fabs(d) > 0.0)) d = 1.0;
-    const double inv = 1.0 / d;
-    __syncthreads();
-    for (int i = tid; i < n; i += 1024) {           // capture column k, then clear it
-        double c = (i == k) ? 0.0 : A[(size_t)i * ld + k];
-        colbuf[i] = c;
-    }
-    __syncthreads();
-    for (int i = tid; i < n; i += 1024) if (i != k) A[(size_t)i * ld + k] = 0.0;
-    for (int j = tid; j < n; j += 1024) {
-        double v = (j == k) ? inv : A[(size_t)k * ld + j] * inv;
-        A[(size_t)k * ld + j] = v;
-        rowbuf[j] = v;
-    }
-}
-
-__global__ void __launch_bounds__(256) gj_update_kernel(double* __restrict__ A, int ld, int n, int k,
-                                                         const double* __restrict__ rowbuf,
-                                                         const double* __restrict__ colbuf) {
-    int j = blockIdx.x * 256 + threadIdx.x;
-    int i0 = blockIdx.y * 16;
-    if (j >= n) return;
-    double r = rowbuf[j];
-#pragma unroll 4
-    for (int ii = 0; ii < 16; ++ii) {
-        int i = i0 + ii;
-        if (i < n && i != k) {
-            double c = colbuf[i];
-            if (c != 0.0) A[(size_t)i * ld + j] -= c * r;
-        }
-    }
-}
-
 __global__ void gj_colswap_kernel(double* __restrict__ A, int ld, int n, const int* __restrict__ piv) {
     // one thread per row: apply the recorded swaps as column swaps in reverse order
     int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -874,7 +784,7 @@ __global__ void __launch_bounds__(256) pack_gform_kernel(const double* __restric
     double* o = out + ((size_t)pm.tile_off[I] + kt) * (KB_BM * KB_BK);
     for (int e = threadIdx.x; e < KB_BM * KB_BK; e += 256) {
         int r, k;
-        pack_rk(true, I, kt, e, r, k);           // fp64 solve kernel order, as pack_kernel<double>
+        pack_rk(I, kt, e, r, k);                 // fp64 solve kernel order, as pack_kernel
         double v = 0.0;
         if (r < n) {
             if (k < r) v = G[(size_t)r * ld + k] + G[(size_t)k * ld + r];
@@ -892,12 +802,13 @@ __global__ void symmetrize_kernel(double* __restrict__ C, int ld, int n_pad) {
 }
 
 // ---------------------------------------------------------------------------
-// Blocked form of the same Gauss-Jordan inversion (the default; the column-at-a-time kernels above stay as the route
-// for devices that cannot co-schedule the panel grid, and as the cross-check of tests/test_parity_gpu.py).
-// 64 scalar steps compose into the block exchange of the pivot block K against the rest R (after the row swaps):
+// Blocked Gauss-Jordan. 64 consecutive column steps of the elimination (step k: pivot search in column k, row swap,
+// scaling of the pivot row, a[i][j] -= a[i][k] a[k][j] for i != k) compose into the block exchange of the pivot block K
+// against the rest R (after the row swaps):
 //     A_KK <- A_KK^-1,  A_RK <- -A_RK A_KK^-1,  A_KR <- A_KK^-1 A_KR,  A_RR <- A_RR - A_RK A_KK^-1 A_KR
-// so one 64-column step is
-//   gj_panel_kernel      the 64 scalar steps with partial pivoting restricted to the n_pad x 64 column panel. The rows
+// (tests/test_host.py::test_blocked_gauss_jordan_algebra pins this against the column steps in numpy), so one 64-column
+// step is
+//   gj_panel_kernel      the 64 column steps with partial pivoting restricted to the n_pad x 64 column panel. The rows
 //                        are dealt to the CTAs of ONE cooperative grid, each CTA keeps its rows of the panel in shared
 //                        memory; per step every CTA publishes its best pivot candidate (|value|, row index, the row's 64
 //                        panel entries) and the owner of row k publishes that row, ONE grid barrier, then every CTA
@@ -905,8 +816,9 @@ __global__ void symmetrize_kernel(double* __restrict__ C, int ld, int n_pad) {
 //                        j+1 separates the reads of step j from the writes of step j+2.
 //   gj_swap_copy_kernel  the recorded row swaps on all other columns, then T = A[K rows][other columns] to a buffer
 //   gj_gemm_kernel       A[:, other] = (rows K: 0, else A[:, other]) + Panel * T   -- rank-64 update on the DMMA pipe
-// i.e. 3 launches and 64 grid barriers per 64 columns instead of 128 launches. The padded rows/columns (identity)
-// take part, so every block is full. Same pivot order, same singularity test as the scalar form.
+// i.e. 3 launches and 64 grid barriers per 64 columns. The padded rows/columns (identity) take part, so every block is
+// full. A pivot at or below ptol is reported as singular: ptol is rounding noise, as the pivot row is scaled, so a
+// redundant row cancels to ~1 ulp, not 0.
 #define GJ_PLD 65
 #define GJ_MAX_CTAS 256
 
@@ -917,12 +829,10 @@ struct GjWork {
     double* cand_val;   // [2][GJ_MAX_CTAS]
     int* cand_idx;      // [2][GJ_MAX_CTAS]
     int* piv;           // [n_pad]
-    double* rowbuf;     // [n_pad]  (scalar form)
-    double* colbuf;     // [n_pad]
 };
 
 size_t kbk_general_inverse_workspace_bytes(int n_pad) {
-    size_t d = (size_t)64 * n_pad + 2 * GJ_MAX_CTAS * 64 + 128 + 2 * GJ_MAX_CTAS + 2 * (size_t)n_pad;
+    size_t d = (size_t)64 * n_pad + 2 * GJ_MAX_CTAS * 64 + 128 + 2 * GJ_MAX_CTAS;
     return d * sizeof(double) + (2 * GJ_MAX_CTAS + (size_t)n_pad + 64) * sizeof(int);
 }
 
@@ -933,8 +843,6 @@ static GjWork gj_carve(void* work, int n_pad) {
     w.cand_row = d; d += 2 * GJ_MAX_CTAS * 64;
     w.krow = d; d += 128;
     w.cand_val = d; d += 2 * GJ_MAX_CTAS;
-    w.rowbuf = d; d += n_pad;
-    w.colbuf = d; d += n_pad;
     int* i = reinterpret_cast<int*>(d);
     w.cand_idx = i; i += 2 * GJ_MAX_CTAS;
     w.piv = i;
@@ -943,7 +851,7 @@ static GjWork gj_carve(void* work, int n_pad) {
 
 static size_t gj_panel_smem(int rpc) { return ((size_t)rpc * (GJ_PLD + 1) + 3 * 64) * sizeof(double); }
 
-// candidates (|v|, row): larger |v| wins, ties go to the lower row index (the scalar form's order)
+// candidates (|v|, row): larger |v| wins, ties go to the lower row index (the first maximum, as LAPACK's getrf)
 __device__ __forceinline__ bool gj_better(double v, int i, double bv, int bi) { return v > bv || (v == bv && i < bi); }
 
 __global__ void __launch_bounds__(256) gj_panel_kernel(double* A, int ld, int n_pad, int k0, int rpc,
@@ -1053,7 +961,7 @@ __global__ void __launch_bounds__(256) gj_panel_kernel(double* A, int ld, int n_
         __syncthreads();
         for (int r = tid; r < R; r += 256) colv[r] = P[r * GJ_PLD + j];
         __syncthreads();
-        // (5) the scalar step on this CTA's rows: row kk becomes the scaled pivot row, column j the negated multipliers
+        // (5) column step kk on this CTA's rows: row kk becomes the scaled pivot row, column j the negated multipliers
         for (int e = tid; e < R * 64; e += 256) {
             const int r = e >> 6, c = e & 63;
             double v;
@@ -1121,40 +1029,30 @@ static int gj_plan(int n_pad, int* rpc_out) {
     return (n_pad + rpc - 1) / rpc;
 }
 
-cudaError_t kbk_general_inverse(double* C, int ld, int n, int n_pad, void* work, int* flag, double ptol,
-                                cudaStream_t st, int* launches, int force_scalar) {
+cudaError_t kbk_general_inverse(double* C, int ld, int n_pad, void* work, int* flag, double ptol,
+                                cudaStream_t st, int* launches) {
     // C holds the assembled lower triangle (+ diagonal, identity in the padding); build the full matrix, then invert
+    int rpc = 0;
+    const int G = gj_plan(n_pad, &rpc);
+    if (G == 0) return cudaErrorNotSupported;
     GjWork w = gj_carve(work, n_pad);
     symmetrize_kernel<<<dim3((n_pad + 255) / 256, n_pad), 256, 0, st>>>(C, ld, n_pad);
     ++*launches;
-    int rpc = 0;
-    const int G = force_scalar ? 0 : gj_plan(n_pad, &rpc);
-    if (G > 0) {
-        const int nbk = n_pad / 64;
-        const size_t smem = gj_panel_smem(rpc);
-        for (int kb = 0; kb < nbk; ++kb) {
-            int k0 = kb * 64;
-            void* args[] = {&C, &ld, &n_pad, &k0, &rpc, &w.cand_row, &w.krow, &w.cand_val, &w.cand_idx, &w.piv, &flag, &ptol};
-            cudaError_t e = cudaLaunchCooperativeKernel((const void*)gj_panel_kernel, dim3(G), dim3(256), args, smem, st);
-            if (e != cudaSuccess) return e;
-            ++*launches;
-            if (nbk > 1) {
-                gj_swap_copy_kernel<<<(n_pad + 255) / 256, 256, 0, st>>>(C, ld, n_pad, k0, w.piv, w.Tbuf);
-                gj_gemm_kernel<<<dim3(nbk, nbk), 128, 0, st>>>(C, ld, n_pad, kb, w.Tbuf);
-                *launches += 2;
-            }
-        }
-        gj_colswap_kernel<<<(n_pad + 127) / 128, 128, 0, st>>>(C, ld, n_pad, w.piv);
+    const int nbk = n_pad / 64;
+    const size_t smem = gj_panel_smem(rpc);
+    for (int kb = 0; kb < nbk; ++kb) {
+        int k0 = kb * 64;
+        void* args[] = {&C, &ld, &n_pad, &k0, &rpc, &w.cand_row, &w.krow, &w.cand_val, &w.cand_idx, &w.piv, &flag, &ptol};
+        KB_CUDA_OK(cudaLaunchCooperativeKernel((const void*)gj_panel_kernel, dim3(G), dim3(256), args, smem, st));
         ++*launches;
-        return cudaGetLastError();
+        if (nbk > 1) {
+            gj_swap_copy_kernel<<<(n_pad + 255) / 256, 256, 0, st>>>(C, ld, n_pad, k0, w.piv, w.Tbuf);
+            gj_gemm_kernel<<<dim3(nbk, nbk), 128, 0, st>>>(C, ld, n_pad, kb, w.Tbuf);
+            *launches += 2;
+        }
     }
-    dim3 ug((n + 255) / 256, (n + 15) / 16);
-    for (int k = 0; k < n; ++k) {
-        gj_pivot_kernel<<<1, 1024, 0, st>>>(C, ld, n, k, w.rowbuf, w.colbuf, w.piv, flag, ptol);
-        gj_update_kernel<<<ug, 256, 0, st>>>(C, ld, n, k, w.rowbuf, w.colbuf);
-    }
-    gj_colswap_kernel<<<(n + 127) / 128, 128, 0, st>>>(C, ld, n, w.piv);
-    *launches += 2 * n + 1;
+    gj_colswap_kernel<<<(n_pad + 127) / 128, 128, 0, st>>>(C, ld, n_pad, w.piv);
+    ++*launches;
     return cudaGetLastError();
 }
 
@@ -1177,9 +1075,6 @@ cudaError_t kbk_dual_gform(const double* G, int ld, int n, int n_pad, int n_rl, 
 
 cudaError_t kbk_pack_gform(const double* G, int ld, int n, int n_pad, int na, const double* Uz,
                            const PackMap& pm, void* out, cudaStream_t st) {
-    int maxkt = 0;
-    for (int i = 0; i < pm.nrb; ++i) maxkt = pm.ktiles[i] > maxkt ? pm.ktiles[i] : maxkt;
-    dim3 grid(maxkt, pm.nrb);
-    pack_gform_kernel<<<grid, 256, 0, st>>>(G, ld, n, n_pad, na, Uz, pm, (double*)out);
+    pack_gform_kernel<<<kb_pack_grid(pm), 256, 0, st>>>(G, ld, n, n_pad, na, Uz, pm, (double*)out);
     return cudaGetLastError();
 }

@@ -1,6 +1,31 @@
 // kernels.h — internal launcher interface between api.cu and the kernel files.
 #pragma once
+#include <type_traits>
 #include "common.cuh"
+
+// Run-time value -> template argument. KbList<V...>::dispatch(v, f) calls f(std::integral_constant<int, V>{}) for the V
+// equal to v and returns its result, cudaErrorInvalidValue if v is not in the list; for_each(f) calls f for every V in
+// order and stops at the first error. Each list is written once, so a case and its template argument cannot disagree.
+template <int... Vs>
+struct KbList {
+    template <typename F>
+    static cudaError_t dispatch(int v, F&& f) {
+        cudaError_t e = cudaErrorInvalidValue;
+        (void)((v == Vs && ((e = f(std::integral_constant<int, Vs>{})), true)) || ...);
+        return e;
+    }
+    template <typename F>
+    static cudaError_t for_each(F&& f) {
+        cudaError_t e = cudaSuccess;
+        (void)(((e = f(std::integral_constant<int, Vs>{})) == cudaSuccess) && ...);
+        return e;
+    }
+};
+using KbDims = KbList<2, 3, KB_GEO>;
+using KbModels = KbList<KB200_VG_LINEAR, KB200_VG_POWER, KB200_VG_GAUSSIAN, KB200_VG_EXPONENTIAL, KB200_VG_SPHERICAL,
+                        KB200_VG_HOLE_EFFECT, KB200_VG_TABLE>;
+using KbSlices = KbList<4, 5, 6>;
+using KbBools = KbList<0, 1>;
 
 struct DriftScale {            // f' = (f - shift) * scale  (change of drift basis)
     double shift[KB200_MAX_DRIFT + 1];
@@ -14,6 +39,12 @@ struct PackMap {
     int ktiles[KB_MAXRB];
     long long tile_off[KB_MAXRB];
 };
+// grid of the pack kernels: CTA (kt, I) packs k tile kt of row block I (and returns if the block has fewer tiles)
+inline dim3 kb_pack_grid(const PackMap& pm) {
+    int maxkt = 0;
+    for (int i = 0; i < pm.nrb; ++i) maxkt = pm.ktiles[i] > maxkt ? pm.ktiles[i] : maxkt;
+    return dim3(maxkt, pm.nrb);
+}
 
 // Drift terms evaluated at the prediction points by the solve kernels themselves (kb200_set_device_drift):
 // point-logarithmic wells (uk.py:955-966) and the external-Z raster with the reference's bilinear sampler
@@ -188,14 +219,16 @@ cudaError_t kbk_dual(const double* W, int ld, int n, int n_pad, int n_rl, int n_
                      const double* ax, const double* ay, const double* az, const DriftScale& ds,
                      const double* hd, const double* values,
                      double* Fz, double* Hz, double* Uz, double* consts, int* flag, cudaStream_t st, int* launches);
-cudaError_t kbk_pack(int dtype, const double* W, int ld, int n, int n_pad, int na, const double* Uz,
+// W (+ dual rows) -> the fp64 tile stream of the DMMA solve kernel
+cudaError_t kbk_pack(const double* W, int ld, int n, int n_pad, int na, const double* Uz,
                      const PackMap& pm, void* out, cudaStream_t st);
 
 // in-place inverse of the (symmetric, possibly indefinite) matrix whose lower triangle is in C: blocked Gauss-Jordan with
-// partial pivoting (cooperative panel kernel + DMMA rank-64 updates); force_scalar = 1 selects the column-at-a-time form
+// partial pivoting (cooperative panel kernel + DMMA rank-64 updates); cudaErrorNotSupported if the device cannot
+// co-schedule the panel grid
 size_t      kbk_general_inverse_workspace_bytes(int n_pad);
-cudaError_t kbk_general_inverse(double* C, int ld, int n, int n_pad, void* work, int* flag, double ptol,
-                                cudaStream_t st, int* launches, int force_scalar);
+cudaError_t kbk_general_inverse(double* C, int ld, int n_pad, void* work, int* flag, double ptol,
+                                cudaStream_t st, int* launches);
 cudaError_t kbk_dual_gform(const double* G, int ld, int n, int n_pad, int n_rl, int n_hd, int nv,
                            const double* ax, const double* ay, const double* az, const DriftScale& ds,
                            const double* hd, const double* values,

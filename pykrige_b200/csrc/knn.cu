@@ -694,36 +694,25 @@ cudaError_t kbk_knn_sort_fields(int n, int nv, const int* sorig, const double* s
     return cudaGetLastError();
 }
 
-template <int DIM, bool CHOL, bool LOO>
-static cudaError_t knn_launch_dim(const KnnParams& p, cudaStream_t st) {
-    size_t per = kbk_knn_smem_per_warp(p.k, CHOL ? 1 : 0, KB_HASZ(DIM) ? 1 : 0, p.nv);
-    int wpc = (int)std::min<size_t>(10, (size_t)(226 * 1024) / per);   // as many points in flight per SM as fit (<= 320 threads; 227 KB minus the static 1 KB)
-    if (wpc < 1) return cudaErrorInvalidValue;
-    size_t smem = per * wpc;
-    unsigned grid = (unsigned)((p.m + wpc - 1) / wpc);
-    int per_d = (int)(per / sizeof(double));
-    switch (p.vg.model) {
-#define KB_CASE(M) case M: { \
-        cudaError_t e = cudaFuncSetAttribute(knn_solve_kernel<DIM, M, CHOL, LOO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-        if (e != cudaSuccess) return e; \
-        knn_solve_kernel<DIM, M, CHOL, LOO><<<grid, wpc * 32, smem, st>>>(p, wpc, per_d); } break;
-        KB_CASE(KB200_VG_LINEAR) KB_CASE(KB200_VG_POWER) KB_CASE(KB200_VG_GAUSSIAN)
-        KB_CASE(KB200_VG_EXPONENTIAL) KB_CASE(KB200_VG_SPHERICAL) KB_CASE(KB200_VG_HOLE_EFFECT) KB_CASE(KB200_VG_TABLE)
-#undef KB_CASE
-        default: return cudaErrorInvalidValue;
-    }
-    return cudaGetLastError();
-}
-
-template <bool LOO>
-static cudaError_t knn_solve_loo(const KnnParams& p, int chol, cudaStream_t st) {
-    if (chol && p.k <= 128)
-        return p.dim == 2 ? knn_launch_dim<2, true, LOO>(p, st) : (p.dim == 3 ? knn_launch_dim<3, true, LOO>(p, st) : knn_launch_dim<KB_GEO, true, LOO>(p, st));
-    return p.dim == 2 ? knn_launch_dim<2, false, LOO>(p, st) : (p.dim == 3 ? knn_launch_dim<3, false, LOO>(p, st) : knn_launch_dim<KB_GEO, false, LOO>(p, st));
-}
-
 cudaError_t kbk_knn_solve(const KnnParams& p, int chol, cudaStream_t st, int loo) {
-    return loo ? knn_solve_loo<true>(p, chol, st) : knn_solve_loo<false>(p, chol, st);
+    return KbDims::dispatch(p.dim, [&](auto D) {
+        return KbModels::dispatch(p.vg.model, [&](auto M) {
+            return KbBools::dispatch(chol && p.k <= 128, [&](auto CHOL) {
+                return KbBools::dispatch(loo != 0, [&](auto LOO) {
+                    const size_t per = kbk_knn_smem_per_warp(p.k, CHOL, KB_HASZ(D) ? 1 : 0, p.nv);
+                    // as many points in flight per SM as fit (<= 320 threads; 227 KB minus the static 1 KB)
+                    const int wpc = (int)std::min<size_t>(10, (size_t)(226 * 1024) / per);
+                    if (wpc < 1) return cudaErrorInvalidValue;
+                    const size_t smem = per * wpc;
+                    KB_CUDA_OK(cudaFuncSetAttribute(knn_solve_kernel<D, M, bool(CHOL), bool(LOO)>,
+                                                    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                    knn_solve_kernel<D, M, bool(CHOL), bool(LOO)><<<(unsigned)((p.m + wpc - 1) / wpc), wpc * 32, smem, st>>>(
+                        p, wpc, (int)(per / sizeof(double)));
+                    return cudaGetLastError();
+                });
+            });
+        });
+    });
 }
 
 cudaError_t kbk_knn_build(int dim, int n, const double* ax, const double* ay, const double* az, const double* values,

@@ -186,11 +186,10 @@ cudaError_t kbk_loo_finalize(const LooParams& p, cudaStream_t st) {
 
 cudaError_t kbk_loo_pairs(int dim, int n, const double* ax, const double* ay, const double* az, double eps, int* cnt,
                           const int* off, int* pj, double* pd, cudaStream_t st) {
-    const int g = (n + 255) / 256;
-    if (dim == KB_GEO) loo_pairs_kernel<KB_GEO><<<g, 256, 0, st>>>(n, ax, ay, az, eps, cnt, off, pj, pd);
-    else if (dim == 3) loo_pairs_kernel<3><<<g, 256, 0, st>>>(n, ax, ay, az, eps, cnt, off, pj, pd);
-    else loo_pairs_kernel<2><<<g, 256, 0, st>>>(n, ax, ay, az, eps, cnt, off, pj, pd);
-    return cudaGetLastError();
+    return KbDims::dispatch(dim, [&](auto D) {
+        loo_pairs_kernel<D><<<(n + 255) / 256, 256, 0, st>>>(n, ax, ay, az, eps, cnt, off, pj, pd);
+        return cudaGetLastError();
+    });
 }
 
 cudaError_t kbk_loo_dup(const LooParams& p, int nst, const int* st_list, const int* off, const int* pj, const double* pd,

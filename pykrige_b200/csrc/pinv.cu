@@ -16,33 +16,11 @@
 
 #define PJ_T 256
 
-// 1-D bulk copies through the TMA engine (SASS UBLKCP): a single CTA per SM cannot keep enough plain
+// 1-D bulk copies through the TMA engine (common.cuh; SASS UBLKCP): a single CTA per SM cannot keep enough plain
 // loads in flight to stream its columns at HBM speed.
-__device__ __forceinline__ uint32_t pj_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void pj_mbar_init(uint64_t* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" :: "r"(pj_smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void pj_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" :: "r"(pj_smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void pj_mbar_wait(uint64_t* bar, uint32_t parity) {
-    for (uint32_t it = 0; it < (1u << 26); ++it) {          // bounded spin: trap instead of hanging the GPU
-        uint32_t ok;
-        asm volatile("{\n\t.reg .pred p;\n\t"
-                     "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-                     "selp.u32 %0, 1, 0, p;\n\t}\n"
-                     : "=r"(ok) : "r"(pj_smem_u32(bar)), "r"(parity) : "memory");
-        if (ok) return;
-    }
-    __trap();
-}
-__device__ __forceinline__ void pj_bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
-                 :: "r"(pj_smem_u32(dst)), "l"(src), "r"(bytes), "r"(pj_smem_u32(bar)) : "memory");
-}
 __device__ __forceinline__ void pj_bulk_s2g(void* dst, const void* src, uint32_t bytes) {
     asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;\n"
-                 :: "l"(dst), "r"(pj_smem_u32(src)), "r"(bytes) : "memory");
+                 :: "l"(dst), "r"(kb_smem_u32(src)), "r"(bytes) : "memory");
 }
 
 // Bt (row p = column p of B) := A, Vt := I. C: assembled with c0 = 0 (lower triangle valid, zero
@@ -109,9 +87,8 @@ __global__ void __launch_bounds__(PJ_T) pinv_jacobi_round_kernel(int nt, int ld,
     if (tid < NC * NC) M[tid / NC][tid % NC] = (tid / NC == tid % NC) ? 1.0 : 0.0;
     if (tid == 0) {
         any_rot = 0;
-        pj_mbar_init(&bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-        asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
+        kb_mbar_init(&bar, 1);
+        kb_fence_mbar_init();
     }
     __syncthreads();
     const int nts = (nt + 1) & ~1;                       // column stride in shared memory (16-byte multiple)
@@ -119,11 +96,11 @@ __global__ void __launch_bounds__(PJ_T) pinv_jacobi_round_kernel(int nt, int ld,
     if (tid == 0) {
         uint32_t total = 0;
         for (int a = 0; a < NC; ++a) if (scol[a] >= 0) total += cb;
-        pj_mbar_expect_tx(&bar, total);
+        kb_mbar_expect_tx(&bar, total);
         for (int a = 0; a < NC; ++a)
-            if (scol[a] >= 0) pj_bulk_g2s(pj_sm + (size_t)a * nts, Bt + (size_t)scol[a] * ld, cb, &bar);
+            if (scol[a] >= 0) kb_bulk_g2s(pj_sm + (size_t)a * nts, Bt + (size_t)scol[a] * ld, cb, &bar);
     }
-    pj_mbar_wait(&bar, 0);
+    kb_mbar_wait(&bar, 0);
     for (int step = 0; step < NC - 1; ++step) {
         // inner round robin on NC players: group 0 pairs (NC-1, step), group g pairs ((step+g), (step-g)) mod NC-1
         int a, c;

@@ -16,36 +16,6 @@
 // The wgmma variants live in solve_tf32.cu (dtype float32) and solve_i8.cu (dtype float64x).
 #include "common.cuh"
 #include "kernels.h"
-#include <cstdlib>
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-    return (uint32_t)__cvta_generic_to_shared(p);
-}
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" :: "r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" :: "r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile("{\n\t.reg .pred p;\n\t"
-                 "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-                 "selp.u32 %0, 1, 0, p;\n\t}\n"
-                 : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-    return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    // bounded spin: a lost transaction traps instead of hanging the GPU
-    for (uint32_t it = 0; it < (1u << 26); ++it)
-        if (mbar_try_wait(bar, parity)) return;
-    __trap();
-}
-// 1-D bulk copy global -> shared through the TMA engine (SASS: UBLKCP)
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
-                 :: "r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
 
 // ---------------------------------------------------------------------------------------------
 // K3 v3: persistent, warp-specialised, one CTA = one tile of 64 prediction points x ALL rows of W.
@@ -69,10 +39,6 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
 #define PT_THREADS 384
 #define PT_CONS0 (PT_THREADS / 32 - 8)    // first of the 8 consumer warps
 #define PT_STAGE_BYTES ((KB_BM * KB_BK + KB_BK * KB_TN) * 8)
-
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" :: "r"(smem_u32(bar)) : "memory");
-}
 
 // Sum of v[0..CNT) over the 8 lanes of a warp that share lane & 3 (the row lanes of an MMA C fragment), halving the
 // values at each of the butterfly steps xor 16, 8, 4: afterwards v[0..max(CNT/8, 1)) hold this lane's share of the sums.
@@ -134,9 +100,8 @@ __global__ void __launch_bounds__(PT_THREADS, 1) solve_kernel_pt(const __grid_co
     const long long ntiles = (P.m + TN - 1) / TN;
 
     if (tid == 0) {
-        for (int s = 0; s < PT_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
-        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-        asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
+        for (int s = 0; s < PT_STAGES; ++s) { kb_mbar_init(&full[s], 1); kb_mbar_init(&empty[s], 8); }
+        kb_fence_mbar_init();
     }
     __syncthreads();
 
@@ -180,9 +145,7 @@ __global__ void __launch_bounds__(PT_THREADS, 1) solve_kernel_pt(const __grid_co
                     dst[1] = make_double2(v[2], v[3]);
                 }
             }
-            // generic-proxy global writes -> later read by the async proxy (bulk copies) of this CTA
-            __threadfence();
-            asm volatile("fence.proxy.async.global;\n" ::: "memory");
+            kb_fence_publish_async();      // the bulk copies of this CTA read the ring
         }
         __syncthreads();
 
@@ -196,8 +159,8 @@ __global__ void __launch_bounds__(PT_THREADS, 1) solve_kernel_pt(const __grid_co
                     const int kt = P.pm.ktiles[I];
                     for (int t = 0; t < kt; ++t, ++tau, ++g) {
                         const int s = g % PT_STAGES;
-                        mbar_wait(&empty[s], (uint32_t)(((g / PT_STAGES) & 1) ^ 1));
-                        mbar_expect_tx(&full[s], (KB_BM * KB_BK + KB_BK * TN) * 8);
+                        kb_mbar_wait(&empty[s], (uint32_t)(((g / PT_STAGES) & 1) ^ 1));
+                        kb_mbar_expect_tx(&full[s], (KB_BM * KB_BK + KB_BK * TN) * 8);
                         kb_bulk_g2s_hint(Ts + (size_t)s * KB_BM * KB_BK, gt + (size_t)tau * (KB_BM * KB_BK),
                                          KB_BM * KB_BK * 8, &full[s], pol_w);
                         kb_bulk_g2s_hint(Bs + (size_t)s * KB_BK * TN, scratch + (size_t)t * (KB_BK * TN),
@@ -243,7 +206,7 @@ __global__ void __launch_bounds__(PT_THREADS, 1) solve_kernel_pt(const __grid_co
                     const int s = g % PT_STAGES;
                     // every consumer waits for every stage (also the ones it skips) so that no warp can lap
                     // the ring and arrive twice on empty[s] within one phase
-                    mbar_wait(&full[s], (uint32_t)((g / PT_STAGES) & 1));
+                    kb_mbar_wait(&full[s], (uint32_t)((g / PT_STAGES) & 1));
                     const bool on0 = g < glim[0], on1 = g < glim[1];
                     if (on0 || on1) {
                         const double2* ts = reinterpret_cast<const double2*>(Ts + (size_t)s * KB_BM * KB_BK);
@@ -265,7 +228,7 @@ __global__ void __launch_bounds__(PT_THREADS, 1) solve_kernel_pt(const __grid_co
                         }
                     }
                     __syncwarp();
-                    if (lane == 0) mbar_arrive(&empty[s]);
+                    if (lane == 0) kb_mbar_arrive(&empty[s]);
                 }
                 // row-block epilogue, in place: every accumulator of a W row becomes its term of the point's sum (square,
                 // or c[r] times it for the quadratic form), dual rows go to shared memory and, like padding rows, add 0;
@@ -353,56 +316,36 @@ size_t kbk_solve_pt_scratch_doubles(int n, int grid) {
 }
 
 
-// The fields kernels run 32- and 16-point tiles only: with 64-point tiles the global staging of the dual rows costs the
-// 64-point kernel its last registers (ptxas spills), so the widest fields tile is NT = 4 (KB_TN_FIELDS in api.cu).
-template <int DIM, int MODEL, bool FIELDS>
-static cudaError_t solve_set_attr_f() {
-    constexpr int NT8 = FIELDS ? 4 : 8;
-    KB_CUDA_OK(cudaFuncSetAttribute(solve_kernel_pt<DIM, MODEL, NT8, FIELDS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)solve_smem_pt()));
-    KB_CUDA_OK(cudaFuncSetAttribute(solve_kernel_pt<DIM, MODEL, 4, FIELDS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)solve_smem_pt()));
-    return cudaFuncSetAttribute(solve_kernel_pt<DIM, MODEL, 2, FIELDS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)solve_smem_pt());
-}
-template <int DIM, int MODEL>
-static cudaError_t solve_set_attr() {
-    KB_CUDA_OK((solve_set_attr_f<DIM, MODEL, false>()));
-    return solve_set_attr_f<DIM, MODEL, true>();
-}
+// Tile widths in points (NT = width / 8 n-tiles). The fields kernels run 32- and 16-point tiles only: with 64-point tiles
+// the global staging of the dual rows costs the 64-point kernel its last registers (ptxas spills), so the widest fields
+// tile is NT = 4 (KB_TN_FIELDS in api.cu).
+using PtWidths = KbList<16, 32, 64>;
 
 cudaError_t kbk_solve_init() {
-#define KB_ATTR(M) KB_CUDA_OK((solve_set_attr<2, M>())); KB_CUDA_OK((solve_set_attr<3, M>())); KB_CUDA_OK((solve_set_attr<KB_GEO, M>()));
-    KB_ATTR(KB200_VG_LINEAR) KB_ATTR(KB200_VG_POWER) KB_ATTR(KB200_VG_GAUSSIAN)
-    KB_ATTR(KB200_VG_EXPONENTIAL) KB_ATTR(KB200_VG_SPHERICAL) KB_ATTR(KB200_VG_HOLE_EFFECT) KB_ATTR(KB200_VG_TABLE)
-#undef KB_ATTR
-    return cudaSuccess;
-}
-
-template <int DIM, bool FIELDS>
-static cudaError_t solve_pt_dim(const SolvePtParams& p, int grid, int tile_points, cudaStream_t st) {
-    size_t sm = solve_smem_pt();
-    constexpr int NT8 = FIELDS ? 4 : 8;
-    if (FIELDS && tile_points == 64) return cudaErrorInvalidValue;
-    switch (p.vg.model) {
-#define KB_CASE(M) case M: if (tile_points == 16) solve_kernel_pt<DIM, M, 2, FIELDS><<<grid, PT_THREADS, sm, st>>>(p); \
-                           else if (tile_points == 32) solve_kernel_pt<DIM, M, 4, FIELDS><<<grid, PT_THREADS, sm, st>>>(p); \
-                           else solve_kernel_pt<DIM, M, NT8, FIELDS><<<grid, PT_THREADS, sm, st>>>(p); break;
-        KB_CASE(KB200_VG_LINEAR) KB_CASE(KB200_VG_POWER) KB_CASE(KB200_VG_GAUSSIAN)
-        KB_CASE(KB200_VG_EXPONENTIAL) KB_CASE(KB200_VG_SPHERICAL) KB_CASE(KB200_VG_HOLE_EFFECT) KB_CASE(KB200_VG_TABLE)
-#undef KB_CASE
-        default: return cudaErrorInvalidValue;
-    }
-    return cudaGetLastError();
+    const int sm = (int)solve_smem_pt();
+    return KbDims::for_each([&](auto D) {
+        return KbModels::for_each([&](auto M) {
+            return PtWidths::for_each([&](auto TN) {
+                KB_CUDA_OK(cudaFuncSetAttribute(solve_kernel_pt<D, M, TN / 8, false>,
+                                                cudaFuncAttributeMaxDynamicSharedMemorySize, sm));
+                if constexpr (TN == 64) return cudaSuccess;
+                else return cudaFuncSetAttribute(solve_kernel_pt<D, M, TN / 8, true>,
+                                                 cudaFuncAttributeMaxDynamicSharedMemorySize, sm);
+            });
+        });
+    });
 }
 
 cudaError_t kbk_solve_pt(int dim, const SolvePtParams& p, int grid, int tile_points, cudaStream_t st) {
-    if (tile_points != 64 && tile_points != 32 && tile_points != 16) return cudaErrorInvalidValue;
-    if (p.nf) {
-        if (dim == KB_GEO) return solve_pt_dim<KB_GEO, true>(p, grid, tile_points, st);
-        return dim == 2 ? solve_pt_dim<2, true>(p, grid, tile_points, st) : solve_pt_dim<3, true>(p, grid, tile_points, st);
-    }
-    if (dim == KB_GEO) return solve_pt_dim<KB_GEO, false>(p, grid, tile_points, st);
-    return dim == 2 ? solve_pt_dim<2, false>(p, grid, tile_points, st) : solve_pt_dim<3, false>(p, grid, tile_points, st);
+    const size_t sm = solve_smem_pt();
+    return KbDims::dispatch(dim, [&](auto D) {
+        return KbModels::dispatch(p.vg.model, [&](auto M) {
+            return PtWidths::dispatch(tile_points, [&](auto TN) {
+                if (!p.nf) solve_kernel_pt<D, M, TN / 8, false><<<grid, PT_THREADS, sm, st>>>(p);
+                else if constexpr (TN == 64) return cudaErrorInvalidValue;
+                else solve_kernel_pt<D, M, TN / 8, true><<<grid, PT_THREADS, sm, st>>>(p);
+                return cudaGetLastError();
+            });
+        });
+    });
 }
-

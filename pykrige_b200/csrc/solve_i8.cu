@@ -27,8 +27,10 @@
 #define I8_BK 32
 #define I8_C_SLICE (I8_TM * I8_BK)            // 2 KB
 
+// W rows per row block: BN / 2 is a valid wgmma N; S * BN / 4 accumulators per thread
+__host__ __device__ constexpr int i8_bn(int S) { return S == 6 ? 48 : 64; }
 template <int S> struct I8Cfg {
-    static constexpr int BN = (S == 6) ? 48 : 64;      // BN / 2 is a valid wgmma N; S * BN / 4 accumulators per thread
+    static constexpr int BN = i8_bn(S);
     static constexpr int STAGES = 6;
     static constexpr int W_SLICE = BN * I8_BK;
     static constexpr int W_BYTES = S * W_SLICE;
@@ -36,27 +38,6 @@ template <int S> struct I8Cfg {
     static constexpr int STAGE_BYTES = W_BYTES + C_BYTES;
 };
 
-__device__ __forceinline__ uint32_t i8_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void i8_mbar_init(uint64_t* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" :: "r"(i8_smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void i8_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" :: "r"(i8_smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void i8_mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" :: "r"(i8_smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void i8_mbar_wait(uint64_t* bar, uint32_t parity) {
-    for (uint32_t it = 0; it < (1u << 26); ++it) {
-        uint32_t ok;
-        asm volatile("{\n\t.reg .pred p;\n\t"
-                     "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-                     "selp.u32 %0, 1, 0, p;\n\t}\n"
-                     : "=r"(ok) : "r"(i8_smem_u32(bar)), "r"(parity) : "memory");
-        if (ok) return;
-    }
-    __trap();
-}
 // K-major, no swizzle: LBO (k-chunk stride) = 128 B, SBO (8-row group stride) = 256 B
 __device__ __forceinline__ uint64_t i8_desc(uint32_t smem_addr) { return kb_wgmma_desc(smem_addr, 128u, 256u); }
 // d[64 points x R*2 W rows] (+)= A[64 x 32] B[R*2 x 32]^T in int32; scale_d = 0 overwrites d
@@ -210,10 +191,9 @@ __global__ void __launch_bounds__(I8_THREADS, 1) solve_kernel_i8(const __grid_co
     const int model = P.vg.model;
 
     if (tid == 0) {
-        for (int s = 0; s < C::STAGES; ++s) { i8_mbar_init(&full[s], 1); i8_mbar_init(&empty[s], 2); }
-        for (int b = 0; b < 2; ++b) { i8_mbar_init(&gfull[b], I8_GEN_THREADS); i8_mbar_init(&gempty[b], 1); }
-        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-        asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
+        for (int s = 0; s < C::STAGES; ++s) { kb_mbar_init(&full[s], 1); kb_mbar_init(&empty[s], 2); }
+        for (int b = 0; b < 2; ++b) { kb_mbar_init(&gfull[b], I8_GEN_THREADS); kb_mbar_init(&gempty[b], 1); }
+        kb_fence_mbar_init();
     }
     __syncthreads();
 
@@ -224,7 +204,7 @@ __global__ void __launch_bounds__(I8_THREADS, 1) solve_kernel_i8(const __grid_co
         uint32_t it = 0;
         for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
             const int b = (int)(it & 1);
-            i8_mbar_wait(&gempty[b], ((it >> 1) & 1) ^ 1);         // the tile that used this buffer is finished
+            kb_mbar_wait(&gempty[b], ((it >> 1) & 1) ^ 1);         // the tile that used this buffer is finished
             unsigned char* sc = scratch + (size_t)b * sbuf;
             const long long pj = tile * I8_TM + pl;
             const bool pvalid = pj < P.m;
@@ -273,10 +253,8 @@ __global__ void __launch_bounds__(I8_THREADS, 1) solve_kernel_i8(const __grid_co
                     }
                 }
             }
-            // generic-proxy global writes -> read by the async proxy (bulk copies) of this CTA
-            __threadfence();
-            asm volatile("fence.proxy.async.global;\n" ::: "memory");
-            i8_mbar_arrive(&gfull[b]);
+            kb_fence_publish_async();      // the bulk copies of this CTA read the ring
+            kb_mbar_arrive(&gfull[b]);
         }
     } else if (warp == 8) {
         // ---------------- producer: W tiles + RHS tiles -> smem ring ----------------
@@ -286,14 +264,14 @@ __global__ void __launch_bounds__(I8_THREADS, 1) solve_kernel_i8(const __grid_co
             for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
                 const int b = (int)(it & 1);
                 const unsigned char* sc = scratch + (size_t)b * sbuf;
-                i8_mbar_wait(&gfull[b], (it >> 1) & 1);
+                kb_mbar_wait(&gfull[b], (it >> 1) & 1);
                 long long tau = 0;
                 for (int J = 0; J < nrb; ++J) {
                     const int kt = i8_ktiles(J, P.n, nk, C::BN);
                     for (int t = 0; t < kt; ++t, ++tau, ++gg) {
                         const int s = gg % C::STAGES;
-                        i8_mbar_wait(&empty[s], (uint32_t)(((gg / C::STAGES) & 1) ^ 1));
-                        i8_mbar_expect_tx(&full[s], C::STAGE_BYTES);
+                        kb_mbar_wait(&empty[s], (uint32_t)(((gg / C::STAGES) & 1) ^ 1));
+                        kb_mbar_expect_tx(&full[s], C::STAGE_BYTES);
                         unsigned char* sb = stage_base + (size_t)s * C::STAGE_BYTES;
                         kb_bulk_g2s_hint(sb, gt + (size_t)tau * C::W_BYTES, C::W_BYTES, &full[s], pol_w);
                         kb_bulk_g2s_hint(sb + C::W_BYTES, sc + (size_t)t * C::C_BYTES, C::C_BYTES, &full[s], pol_c);
@@ -311,7 +289,7 @@ __global__ void __launch_bounds__(I8_THREADS, 1) solve_kernel_i8(const __grid_co
         uint32_t gg = 0, it = 0;
         for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
             const int b = (int)(it & 1);
-            i8_mbar_wait(&gfull[b], (it >> 1) & 1);            // acquire the generators' pexp[b]
+            kb_mbar_wait(&gfull[b], (it >> 1) & 1);            // acquire the generators' pexp[b]
             double pscale[2];
             for (int hh = 0; hh < 2; ++hh) pscale[hh] = scalbn(1.0, pexp[b * I8_TM + p0 + 8 * hh] - 7 * (S - 1));
             double q[2] = {0.0, 0.0};
@@ -320,10 +298,10 @@ __global__ void __launch_bounds__(I8_THREADS, 1) solve_kernel_i8(const __grid_co
                 uint32_t acc[S][R];
                 for (int t = 0; t < kt; ++t, ++gg) {
                     const int s = gg % C::STAGES;
-                    i8_mbar_wait(&full[s], (uint32_t)((gg / C::STAGES) & 1));
+                    kb_mbar_wait(&full[s], (uint32_t)((gg / C::STAGES) & 1));
                     kb_wgmma_fence();
-                    const uint32_t wb = i8_smem_u32(stage_base + (size_t)s * C::STAGE_BYTES) + hoff;
-                    const uint32_t cb = i8_smem_u32(stage_base + (size_t)s * C::STAGE_BYTES) + C::W_BYTES;
+                    const uint32_t wb = kb_smem_u32(stage_base + (size_t)s * C::STAGE_BYTES) + hoff;
+                    const uint32_t cb = kb_smem_u32(stage_base + (size_t)s * C::STAGE_BYTES) + C::W_BYTES;
 #pragma unroll
                     for (int d = 0; d < S; ++d) {
 #pragma unroll
@@ -335,10 +313,10 @@ __global__ void __launch_bounds__(I8_THREADS, 1) solve_kernel_i8(const __grid_co
                     }
                     kb_wgmma_commit();
                     kb_wgmma_wait<1>();                  // the previous stage has been read: hand it back
-                    if (t > 0 && wtid == 0) i8_mbar_arrive(&empty[(gg - 1) % C::STAGES]);
+                    if (t > 0 && wtid == 0) kb_mbar_arrive(&empty[(gg - 1) % C::STAGES]);
                 }
                 kb_wgmma_wait<0>();
-                if (wtid == 0) i8_mbar_arrive(&empty[(gg - 1) % C::STAGES]);
+                if (wtid == 0) kb_mbar_arrive(&empty[(gg - 1) % C::STAGES]);
 #pragma unroll
                 for (int d = 0; d < S; ++d)
 #pragma unroll
@@ -373,7 +351,7 @@ __global__ void __launch_bounds__(I8_THREADS, 1) solve_kernel_i8(const __grid_co
                 if (pj < P.m) kb_finalize_point<DIM, double>(P, pj, qpart[tid] + qpart[I8_TM + tid], auxs + tid, I8_TM);
             }
             kb_named_sync(1, I8_CONS_THREADS);
-            if (tid == 0) i8_mbar_arrive(&gempty[b]);       // scratch half b and pexp[b] may be rewritten
+            if (tid == 0) kb_mbar_arrive(&gempty[b]);       // scratch half b and pexp[b] may be rewritten
         }
     }
 }
@@ -383,8 +361,7 @@ template <int S> static size_t i8_smem_s() {
     return (size_t)I8Cfg<S>::STAGES * I8Cfg<S>::STAGE_BYTES + (size_t)KB_MAXAUX * I8_TM * sizeof(double) +
            2 * I8_TM * sizeof(double) + 2 * I8_TM * sizeof(int) + (2 * I8Cfg<S>::STAGES + 4) * sizeof(uint64_t) + 64;
 }
-static int i8_bn(int S) { return S == 6 ? I8Cfg<6>::BN : S == 5 ? I8Cfg<5>::BN : I8Cfg<4>::BN; }
-bool kbk_i8_valid_slices(int S) { return S >= 4 && S <= 6; }
+bool kbk_i8_valid_slices(int S) { return KbSlices::dispatch(S, [](auto) { return cudaSuccess; }) == cudaSuccess; }
 int kbk_i8_nrb(int S, int n, int na) { return (n + na + i8_bn(S) - 1) / i8_bn(S); }
 int kbk_i8_rows(int S, int n, int na) { return kbk_i8_nrb(S, n, na) * i8_bn(S); }
 long long kbk_i8_total_tiles(int S, int n, int na, long long* tile_off /* [nrb+1] or null */) {
@@ -398,28 +375,22 @@ size_t kbk_i8_tile_bytes(int S) { return (size_t)S * i8_bn(S) * I8_BK; }
 size_t kbk_solve_i8_scratch_bytes(int S, int n, int grid) { return (size_t)grid * 2 * ((n + I8_BK - 1) / I8_BK) * S * I8_C_SLICE; }   // double-buffered
 int kbk_solve_i8_tile_points() { return I8_TM; }
 
-template <int S, int DIM>
-static cudaError_t i8_attr() {
-    return cudaFuncSetAttribute(solve_kernel_i8<S, DIM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)i8_smem_s<S>());
-}
 cudaError_t kbk_solve_i8_init() {
-#define KB_ATTR(S) KB_CUDA_OK((i8_attr<S, 2>())); KB_CUDA_OK((i8_attr<S, 3>())); KB_CUDA_OK((i8_attr<S, KB_GEO>()));
-    KB_ATTR(4) KB_ATTR(5) KB_ATTR(6)
-#undef KB_ATTR
-    return cudaSuccess;
+    return KbSlices::for_each([](auto S) {
+        return KbDims::for_each([&](auto D) {
+            return cudaFuncSetAttribute(solve_kernel_i8<S, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)i8_smem_s<S>());
+        });
+    });
 }
 
-template <int S>
-static cudaError_t i8_launch(int dim, const SolvePtParams& p, int grid, cudaStream_t st) {
-    const size_t sm = i8_smem_s<S>();
-    if (dim == KB_GEO) solve_kernel_i8<S, KB_GEO><<<grid, I8_THREADS, sm, st>>>(p);
-    else if (dim == 2) solve_kernel_i8<S, 2><<<grid, I8_THREADS, sm, st>>>(p);
-    else solve_kernel_i8<S, 3><<<grid, I8_THREADS, sm, st>>>(p);
-    return cudaGetLastError();
-}
 cudaError_t kbk_solve_i8(int S, int dim, const SolvePtParams& p, int grid, cudaStream_t st) {
     if (p.vg.model < KB200_VG_LINEAR || p.vg.model > KB200_VG_TABLE) return cudaErrorInvalidValue;
-    return S == 6 ? i8_launch<6>(dim, p, grid, st) : S == 5 ? i8_launch<5>(dim, p, grid, st) : i8_launch<4>(dim, p, grid, st);
+    return KbSlices::dispatch(S, [&](auto SL) {
+        return KbDims::dispatch(dim, [&](auto D) {
+            solve_kernel_i8<SL, D><<<grid, I8_THREADS, i8_smem_s<SL>(), st>>>(p);
+            return cudaGetLastError();
+        });
+    });
 }
 
 // W (+ dual rows) -> row scales + int8 slice tiles. tile_off_dev: device copy of the per-row-block tile offsets.
@@ -428,9 +399,8 @@ cudaError_t kbk_pack_i8(int S, const double* W, int ld, int n, int n_pad, int na
     int nrb = kbk_i8_nrb(S, n, na), nk = (n + I8_BK - 1) / I8_BK;
     int nrows = nrb * i8_bn(S);
     i8_rowscale_kernel<<<(nrows + 7) / 8, 256, 0, st>>>(W, ld, n, n_pad, na, Uz, nrows, rowexp, rowscale);
-    dim3 grid(nk, nrb);
-    if (S == 6) i8_pack_kernel<6><<<grid, 256, 0, st>>>(W, ld, n, n_pad, na, Uz, rowexp, nk, tile_off_dev, (signed char*)out);
-    else if (S == 5) i8_pack_kernel<5><<<grid, 256, 0, st>>>(W, ld, n, n_pad, na, Uz, rowexp, nk, tile_off_dev, (signed char*)out);
-    else i8_pack_kernel<4><<<grid, 256, 0, st>>>(W, ld, n, n_pad, na, Uz, rowexp, nk, tile_off_dev, (signed char*)out);
-    return cudaGetLastError();
+    return KbSlices::dispatch(S, [&](auto SL) {
+        i8_pack_kernel<SL><<<dim3(nk, nrb), 256, 0, st>>>(W, ld, n, n_pad, na, Uz, rowexp, nk, tile_off_dev, (signed char*)out);
+        return cudaGetLastError();
+    });
 }

@@ -27,27 +27,6 @@
 #define TF_C_BYTES (TF_TM * TF_BK * 4 * 2)     // hi + lo = 8 KB
 #define TF_STAGE_BYTES (TF_W_BYTES + TF_C_BYTES)
 
-__device__ __forceinline__ uint32_t tf_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void tf_mbar_init(uint64_t* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" :: "r"(tf_smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void tf_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" :: "r"(tf_smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tf_mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" :: "r"(tf_smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tf_mbar_wait(uint64_t* bar, uint32_t parity) {
-    for (uint32_t it = 0; it < (1u << 26); ++it) {
-        uint32_t ok;
-        asm volatile("{\n\t.reg .pred p;\n\t"
-                     "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-                     "selp.u32 %0, 1, 0, p;\n\t}\n"
-                     : "=r"(ok) : "r"(tf_smem_u32(bar)), "r"(parity) : "memory");
-        if (ok) return;
-    }
-    __trap();     // a lost arrival traps instead of hanging the GPU
-}
 __device__ __forceinline__ float tf32_round(float x) {
     uint32_t u;
     asm("cvt.rna.tf32.f32 %0, %1;\n" : "=r"(u) : "f"(x));
@@ -135,10 +114,9 @@ __global__ void __launch_bounds__(TF_THREADS, 1) solve_kernel_tf32(const __grid_
     const long long ntiles = (P.m + TF_TM - 1) / TF_TM;
 
     if (tid == 0) {
-        for (int s = 0; s < TF_STAGES; ++s) { tf_mbar_init(&full[s], 1); tf_mbar_init(&empty[s], 2); }
-        for (int b = 0; b < 2; ++b) { tf_mbar_init(&gfull[b], TF_GEN_THREADS); tf_mbar_init(&gempty[b], 1); }
-        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-        asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
+        for (int s = 0; s < TF_STAGES; ++s) { kb_mbar_init(&full[s], 1); kb_mbar_init(&empty[s], 2); }
+        for (int b = 0; b < 2; ++b) { kb_mbar_init(&gfull[b], TF_GEN_THREADS); kb_mbar_init(&gempty[b], 1); }
+        kb_fence_mbar_init();
     }
     __syncthreads();
 
@@ -151,7 +129,7 @@ __global__ void __launch_bounds__(TF_THREADS, 1) solve_kernel_tf32(const __grid_
         uint32_t it = 0;
         for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
             const int b = (int)(it & 1);
-            tf_mbar_wait(&gempty[b], ((it >> 1) & 1) ^ 1);
+            kb_mbar_wait(&gempty[b], ((it >> 1) & 1) ^ 1);
             unsigned char* sc = scratch + (size_t)b * sbuf;
             const long long pj = tile * TF_TM + pl;
             const bool pvalid = pj < P.m;
@@ -179,9 +157,8 @@ __global__ void __launch_bounds__(TF_THREADS, 1) solve_kernel_tf32(const __grid_
                     *reinterpret_cast<float4*>(ct + TF_TM * TF_BK + off) = make_float4(lo[0], lo[1], lo[2], lo[3]);
                 }
             }
-            __threadfence();
-            asm volatile("fence.proxy.async.global;\n" ::: "memory");
-            tf_mbar_arrive(&gfull[b]);
+            kb_fence_publish_async();
+            kb_mbar_arrive(&gfull[b]);
         }
     } else if (warp == 8) {
         if (lane == 0) {
@@ -190,14 +167,14 @@ __global__ void __launch_bounds__(TF_THREADS, 1) solve_kernel_tf32(const __grid_
             for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
                 const int b = (int)(it & 1);
                 const unsigned char* sc = scratch + (size_t)b * sbuf;
-                tf_mbar_wait(&gfull[b], (it >> 1) & 1);
+                kb_mbar_wait(&gfull[b], (it >> 1) & 1);
                 long long tau = 0;
                 for (int I = 0; I < P.nrb; ++I) {
                     const int kt = P.pm.ktiles[I];
                     for (int t = 0; t < kt; ++t, ++tau, ++gg) {
                         const int s = gg % TF_STAGES;
-                        tf_mbar_wait(&empty[s], (uint32_t)(((gg / TF_STAGES) & 1) ^ 1));
-                        tf_mbar_expect_tx(&full[s], TF_STAGE_BYTES);
+                        kb_mbar_wait(&empty[s], (uint32_t)(((gg / TF_STAGES) & 1) ^ 1));
+                        kb_mbar_expect_tx(&full[s], TF_STAGE_BYTES);
                         unsigned char* sb = stage_base + (size_t)s * TF_STAGE_BYTES;
                         kb_bulk_g2s_hint(sb, gt + (size_t)tau * TF_W_BYTES, TF_W_BYTES, &full[s], pol_w);
                         kb_bulk_g2s_hint(sb + TF_W_BYTES, sc + (size_t)t * TF_C_BYTES, TF_C_BYTES, &full[s], pol_c);
@@ -221,9 +198,9 @@ __global__ void __launch_bounds__(TF_THREADS, 1) solve_kernel_tf32(const __grid_
                 float acc[64];
                 for (int t = 0; t < kt; ++t, ++gg) {
                     const int s = gg % TF_STAGES;
-                    tf_mbar_wait(&full[s], (uint32_t)((gg / TF_STAGES) & 1));
+                    kb_mbar_wait(&full[s], (uint32_t)((gg / TF_STAGES) & 1));
                     kb_wgmma_fence();
-                    const uint32_t wb = tf_smem_u32(stage_base + (size_t)s * TF_STAGE_BYTES);
+                    const uint32_t wb = kb_smem_u32(stage_base + (size_t)s * TF_STAGE_BYTES);
                     const uint32_t w_hi = wb + hoff, w_lo = wb + TF_W_BYTES / 2 + hoff;
                     const uint32_t c_hi = wb + TF_W_BYTES, c_lo = c_hi + TF_C_BYTES / 2;
 #pragma unroll
@@ -235,10 +212,10 @@ __global__ void __launch_bounds__(TF_THREADS, 1) solve_kernel_tf32(const __grid_
                     }
                     kb_wgmma_commit();
                     kb_wgmma_wait<1>();                  // the previous stage has been read: hand it back
-                    if (t > 0 && wtid == 0) tf_mbar_arrive(&empty[(gg - 1) % TF_STAGES]);
+                    if (t > 0 && wtid == 0) kb_mbar_arrive(&empty[(gg - 1) % TF_STAGES]);
                 }
                 kb_wgmma_wait<0>();
-                if (wtid == 0) tf_mbar_arrive(&empty[(gg - 1) % TF_STAGES]);
+                if (wtid == 0) kb_mbar_arrive(&empty[(gg - 1) % TF_STAGES]);
 #pragma unroll
                 for (int i = 0; i < 64; ++i) kb_reg_fence(acc[i]);
                 const int rb = I * TF_BN + c0;
@@ -269,7 +246,7 @@ __global__ void __launch_bounds__(TF_THREADS, 1) solve_kernel_tf32(const __grid_
                 if (pj < P.m) kb_finalize_point<DIM, float>(P, pj, qpart[tid] + qpart[TF_TM + tid], auxs + tid, TF_TM);
             }
             kb_named_sync(1, TF_CONS_THREADS);
-            if (tid == 0) tf_mbar_arrive(&gempty[(int)(it & 1)]);      // this tile's scratch half may be rewritten
+            if (tid == 0) kb_mbar_arrive(&gempty[(int)(it & 1)]);      // this tile's scratch half may be rewritten
         }
     }
 }
@@ -285,42 +262,25 @@ size_t kbk_solve_tf32_scratch_bytes(int n, int grid) {
 }
 int kbk_solve_tf32_tile_points() { return TF_TM; }
 
-template <int DIM, int MODEL>
-static cudaError_t tf32_attr() {
-    return cudaFuncSetAttribute(solve_kernel_tf32<DIM, MODEL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tf32_smem());
-}
-
 cudaError_t kbk_solve_tf32_init() {
-#define KB_ATTR(M) KB_CUDA_OK((tf32_attr<2, M>())); KB_CUDA_OK((tf32_attr<3, M>())); KB_CUDA_OK((tf32_attr<KB_GEO, M>()));
-    KB_ATTR(KB200_VG_LINEAR) KB_ATTR(KB200_VG_POWER) KB_ATTR(KB200_VG_GAUSSIAN)
-    KB_ATTR(KB200_VG_EXPONENTIAL) KB_ATTR(KB200_VG_SPHERICAL) KB_ATTR(KB200_VG_HOLE_EFFECT) KB_ATTR(KB200_VG_TABLE)
-#undef KB_ATTR
-    return cudaSuccess;
-}
-
-template <int DIM>
-static cudaError_t tf32_dim(const SolvePtParams& p, int grid, cudaStream_t st) {
-    size_t sm = tf32_smem();
-    switch (p.vg.model) {
-#define KB_CASE(M) case M: solve_kernel_tf32<DIM, M><<<grid, TF_THREADS, sm, st>>>(p); break;
-        KB_CASE(KB200_VG_LINEAR) KB_CASE(KB200_VG_POWER) KB_CASE(KB200_VG_GAUSSIAN)
-        KB_CASE(KB200_VG_EXPONENTIAL) KB_CASE(KB200_VG_SPHERICAL) KB_CASE(KB200_VG_HOLE_EFFECT) KB_CASE(KB200_VG_TABLE)
-#undef KB_CASE
-        default: return cudaErrorInvalidValue;
-    }
-    return cudaGetLastError();
+    return KbDims::for_each([&](auto D) {
+        return KbModels::for_each([&](auto M) {
+            return cudaFuncSetAttribute(solve_kernel_tf32<D, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tf32_smem());
+        });
+    });
 }
 
 cudaError_t kbk_solve_tf32(int dim, const SolvePtParams& p, int grid, cudaStream_t st) {
-    if (dim == KB_GEO) return tf32_dim<KB_GEO>(p, grid, st);
-    return dim == 2 ? tf32_dim<2>(p, grid, st) : tf32_dim<3>(p, grid, st);
+    return KbDims::dispatch(dim, [&](auto D) {
+        return KbModels::dispatch(p.vg.model, [&](auto M) {
+            solve_kernel_tf32<D, M><<<grid, TF_THREADS, tf32_smem(), st>>>(p);
+            return cudaGetLastError();
+        });
+    });
 }
 
 cudaError_t kbk_pack_tf32(const double* W, int ld, int n, int n_pad, int na, const double* Uz, const PackMap& pm,
                           void* out, cudaStream_t st) {
-    int maxkt = 0;
-    for (int i = 0; i < pm.nrb; ++i) maxkt = pm.ktiles[i] > maxkt ? pm.ktiles[i] : maxkt;
-    dim3 grid(maxkt, pm.nrb);
-    pack_tf32_kernel<<<grid, 256, 0, st>>>(W, ld, n, n_pad, na, Uz, pm, (float*)out);
+    pack_tf32_kernel<<<kb_pack_grid(pm), 256, 0, st>>>(W, ld, n, n_pad, na, Uz, pm, (float*)out);
     return cudaGetLastError();
 }

@@ -173,14 +173,10 @@ size_t kbk_ev_smem(int nlags, int priv) {
 int kbk_ev_priv_max_lags() { return (int)((227 * 1024 - (4 * EV_J + 2) * 8) / ((3 * EV_T + 1) * 8)); }
 
 cudaError_t kbk_ev_init() {
-    const int mx = 227 * 1024;
-    cudaError_t e;
-#define KB_EVATTR(D) \
-    if ((e = cudaFuncSetAttribute(ev_bin_kernel<D, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx)) != cudaSuccess) return e; \
-    if ((e = cudaFuncSetAttribute(ev_bin_kernel<D, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, mx)) != cudaSuccess) return e;
-    KB_EVATTR(2) KB_EVATTR(3) KB_EVATTR(KB_GEO)
-#undef KB_EVATTR
-    return cudaSuccess;
+    return KbDims::for_each([](auto D) {
+        KB_CUDA_OK(cudaFuncSetAttribute(ev_bin_kernel<D, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        return cudaFuncSetAttribute(ev_bin_kernel<D, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    });
 }
 
 int kbk_ev_grid(int n, int num_sms) {
@@ -190,11 +186,10 @@ int kbk_ev_grid(int n, int num_sms) {
 
 cudaError_t kbk_ev_minmax(int dim, int n, const double* x, const double* y, const double* z, int grid,
                           double* bmin, double* bmax, cudaStream_t st) {
-    const long long nt = ev_ntiles(n);
-    if (dim == KB_GEO) ev_minmax_kernel<KB_GEO><<<grid, EV_T, 0, st>>>(n, x, y, z, nt, bmin, bmax);
-    else if (dim == 3) ev_minmax_kernel<3><<<grid, EV_T, 0, st>>>(n, x, y, z, nt, bmin, bmax);
-    else ev_minmax_kernel<2><<<grid, EV_T, 0, st>>>(n, x, y, z, nt, bmin, bmax);
-    return cudaGetLastError();
+    return KbDims::dispatch(dim, [&](auto D) {
+        ev_minmax_kernel<D><<<grid, EV_T, 0, st>>>(n, x, y, z, ev_ntiles(n), bmin, bmax);
+        return cudaGetLastError();
+    });
 }
 
 cudaError_t kbk_ev_bin(int dim, int n, const double* x, const double* y, const double* z, const double* v,
@@ -203,13 +198,12 @@ cudaError_t kbk_ev_bin(int dim, int n, const double* x, const double* y, const d
     const long long nt = ev_ntiles(n);
     const int priv = nlags <= kbk_ev_priv_max_lags();
     const size_t sm = kbk_ev_smem(nlags, priv);
-#define KB_EVBIN(D) do { \
-        if (priv) ev_bin_kernel<D, true><<<grid, EV_T, sm, st>>>(n, x, y, z, v, nt, nlags, edges, inv_dd, part); \
-        else ev_bin_kernel<D, false><<<grid, EV_T, sm, st>>>(n, x, y, z, v, nt, nlags, edges, inv_dd, part); } while (0)
-    if (dim == KB_GEO) KB_EVBIN(KB_GEO); else if (dim == 3) KB_EVBIN(3); else KB_EVBIN(2);
-#undef KB_EVBIN
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
+    KB_CUDA_OK(KbDims::dispatch(dim, [&](auto D) {
+        return KbBools::dispatch(priv, [&](auto PRIV) {
+            ev_bin_kernel<D, bool(PRIV)><<<grid, EV_T, sm, st>>>(n, x, y, z, v, nt, nlags, edges, inv_dd, part);
+            return cudaGetLastError();
+        });
+    }));
     ev_reduce_kernel<<<(3 * nlags + 127) / 128, 128, 0, st>>>(grid, nlags, part, out);
     return cudaGetLastError();
 }
@@ -280,13 +274,11 @@ cudaError_t kbk_statistics(int dim, int n, const double* ax, const double* ay, c
                            double* delta, double* sigma, cudaStream_t st) {
     const int gb = (n + 255) / 256;
     const dim3 g(gb, gb);
-    cudaError_t e = cudaMemsetAsync(dup, 0, (size_t)n * sizeof(int), st);
-    if (e != cudaSuccess) return e;
-    if (dim == KB_GEO) stats_dup_kernel<KB_GEO><<<g, 256, 0, st>>>(n, ax, ay, az, dup);
-    else if (dim == 3) stats_dup_kernel<3><<<g, 256, 0, st>>>(n, ax, ay, az, dup);
-    else stats_dup_kernel<2><<<g, 256, 0, st>>>(n, ax, ay, az, dup);
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
+    KB_CUDA_OK(cudaMemsetAsync(dup, 0, (size_t)n * sizeof(int), st));
+    KB_CUDA_OK(KbDims::dispatch(dim, [&](auto D) {
+        stats_dup_kernel<D><<<g, 256, 0, st>>>(n, ax, ay, az, dup);
+        return cudaGetLastError();
+    }));
     stats_kernel<<<1, 1024, 0, st>>>(n, L, ld, u, zeta, dup, delta, sigma);
     return cudaGetLastError();
 }

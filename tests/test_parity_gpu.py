@@ -296,11 +296,12 @@ def test_indefinite_variogram_takes_general_path(pk, ref_cases):
         ok.execute("points", pts[:4, 0], pts[:4, 1], backend="cuda", dtype="float32")
 
 
-def test_blocked_general_inverse_matches_scalar_form_and_oracle(pk, monkeypatch):
+def test_blocked_general_inverse_matches_refined_reference_and_oracle(pk):
     """The general path's inverse is a blocked Gauss-Jordan (cooperative panel kernel + DMMA rank-64 updates). At a
-    size with many panels (N = 1900 -> 30 panels, rows dealt over the whole grid) it must reproduce the oracle's
-    LU-based numbers (ok.py:663) and the column-at-a-time form of the same elimination (KB200_GJ=scalar), for OK
-    and for UK; redundant points must still be reported as singular, not inverted into noise."""
+    size with many panels (N = 1900 -> n_pad = 2048, 32 panels, rows dealt over the whole grid) it must reproduce the
+    oracle's LU-based numbers (ok.py:663) for OK and UK, and the extended-precision solution of the same system
+    (oracle.krige_oracle.exec_vector_refined) to 1e-7, in a fixed number of launches; redundant points must still be
+    reported as singular, not inverted into noise."""
     from oracle import krige_oracle as ko
     xyz, val = cases.synth_data(21, 1900, 2)
     params = [1.0, 250.0, 0.02]
@@ -308,24 +309,25 @@ def test_blocked_general_inverse_matches_scalar_form_and_oracle(pk, monkeypatch)
     sp = ko.stored_parameters("hole-effect", params)
     zo, so = ko.krige(xyz, val, "hole-effect", sp, pts)
     zu, su = ko.krige(xyz, val, "hole-effect", sp, pts, regional_linear=True)
-    out, launches = {}, {}
-    for mode in ("blocked", "scalar"):
-        monkeypatch.setenv("KB200_GJ", mode)
-        ok = pk.OrdinaryKriging(xyz[:, 0], xyz[:, 1], val, variogram_model="hole-effect", variogram_parameters=params)
-        z, ss = ok.execute("points", pts[:, 0], pts[:, 1], backend="cuda")
-        launches[mode] = ok._kb_handle.timings()["launches"]
-        assert_parity(z, zo, R64, "blocked GJ z (scalar=%s)" % mode)
-        assert_parity(ss, so, R64, "blocked GJ ss (scalar=%s)" % mode)
-        out[mode] = (z, ss)
-        uk = pk.UniversalKriging(xyz[:, 0], xyz[:, 1], val, variogram_model="hole-effect", variogram_parameters=params,
-                                 drift_terms=["regional_linear"])
-        z, ss = uk.execute("points", pts[:, 0], pts[:, 1], backend="cuda")
-        assert_parity(z, zu, R64, "blocked GJ uk z (scalar=%s)" % mode)
-        assert_parity(ss, su, R64, "blocked GJ uk ss (scalar=%s)" % mode)
-    assert launches["blocked"] + 3000 < launches["scalar"]          # 3 launches per 64 columns instead of 2 per column
-    assert_parity(out["blocked"][0], out["scalar"][0], 1e-7, "blocked vs scalar z")
-    assert_parity(out["blocked"][1], out["scalar"][1], 1e-7, "blocked vs scalar ss")
-    monkeypatch.setenv("KB200_GJ", "blocked")
+    ok = pk.OrdinaryKriging(xyz[:, 0], xyz[:, 1], val, variogram_model="hole-effect", variogram_parameters=params)
+    z, ss = ok.execute("points", pts[:, 0], pts[:, 1], backend="cuda")
+    assert_parity(z, zo, R64, "blocked GJ z")
+    assert_parity(ss, so, R64, "blocked GJ ss")
+    center = (xyz.max(axis=0) + xyz.min(axis=0)) / 2.0
+    P = ko.adjust_for_anisotropy(xyz, center, [1.0], [0.0])
+    Q = ko.adjust_for_anisotropy(pts, center, [1.0], [0.0])
+    zr, sr, _ = ko.exec_vector_refined(ko.kriging_matrix(P, "hole-effect", sp), P, Q, val, "hole-effect", sp)
+    assert_parity(z, zr, 1e-7, "blocked GJ z vs refined")
+    assert_parity(ss, sr, 1e-7, "blocked GJ ss vs refined")
+    # n_pad = 2048 is 32 blocks of 64: adjust 1 + assemble 1 + the Cholesky that finds C indefinite 46 (32 panels,
+    # 7 look-ahead and 6 trailing updates, 1 diagonal write-back) + assemble 1 + inverse 98 (symmetrize 1, 3 per 64
+    # columns, column swaps 1) + dual 3 + pack 1 + solve 1 (500 points: one launch)
+    assert ok._kb_handle.timings()["launches"] == 152
+    uk = pk.UniversalKriging(xyz[:, 0], xyz[:, 1], val, variogram_model="hole-effect", variogram_parameters=params,
+                             drift_terms=["regional_linear"])
+    z, ss = uk.execute("points", pts[:, 0], pts[:, 1], backend="cuda")
+    assert_parity(z, zu, R64, "blocked GJ uk z")
+    assert_parity(ss, su, R64, "blocked GJ uk ss")
     dup = np.vstack([xyz[:700], xyz[:4]])
     okd = pk.OrdinaryKriging(dup[:, 0], dup[:, 1], np.concatenate([val[:700], val[:4]]), variogram_model="hole-effect",
                              variogram_parameters=[1.0, 250.0, 0.0])
