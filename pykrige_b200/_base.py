@@ -1,16 +1,30 @@
 """Shared host logic of the four kriging classes (not part of the reference's API surface).
 
-The reference repeats this logic in ok.py / uk.py / ok3d.py / uk3d.py; here it lives once:
-variogram model selection (ok.py:208-253), the ``backend='cuda'`` dispatch that replaces the
-``backend`` string switch of ``execute`` (ok.py:971-1010), point-list / grid / mask handling
-(ok.py:842-900, ok3d.py:833-898) and output shaping (ok.py:1012-1020).
+The reference repeats this logic in ok.py / uk.py / ok3d.py / uk3d.py; here it lives once, for 2-D and 3-D alike:
+the constructor and update_variogram_model (ok.py:208-553, uk.py:246-790, ok3d.py:221-520, uk3d.py:239-660),
+variogram model selection (ok.py:208-253), the ``backend='cuda'`` dispatch that replaces the ``backend`` string switch
+of ``execute`` (ok.py:971-1010), point-list / grid / mask handling (ok.py:842-900, ok3d.py:833-898), the 'specified'
+and 'functional' drift terms of the universal classes and output shaping (ok.py:1012-1020). What differs between the
+dimensions and the classes is data: the class attributes of Krige2D / Krige3D and of the four classes.
 """
+import hashlib
 import warnings
+from collections import namedtuple
+
 import numpy as np
 
 from . import variogram_models
 from . import core
 from . import _cabi
+from .core import _adjust_for_anisotropy, _make_variogram_parameter_list, _initialize_variogram_model
+
+P_INV_TYPES = ("pinv", "pinvh")
+GEO_ANISOTROPY_WARNING = "Anisotropy is not compatible with geographic coordinates. Ignoring user set anisotropy."
+
+# What the device problem on a handle was built from. digest covers every input array (coordinates, values, host drift
+# columns, device drift arrays, value fields), so that an in-place edit of any of them invalidates the factorisation.
+ProblemKey = namedtuple("ProblemKey", "dtype knn model params exact_values aniso center n_rl geographic pseudo_inv "
+                                      "n_fields digest")
 
 
 class KrigeBase:
@@ -23,20 +37,43 @@ class KrigeBase:
         "exponential": variogram_models.exponential_variogram_model,
         "hole-effect": variogram_models.hole_effect_variogram_model,
     }
-    _ndim = 2
+    # per dimension (Krige2D / Krige3D): coordinate letters (X_ORIG, XCENTER, X_ADJUSTED, ...), the attribute of the
+    # values, the anisotropy attributes (scalings, then angles: the order of the constructor's arguments)
+    _ndim = None
+    _AXES = None
+    _VALUES = None
+    _SCALINGS = ()
+    _ANGLES = ()
+    # per class: the name in the backend error, drift terms (the universal classes), whether n_closest_points is checked
+    # before the point lists (OrdinaryKriging), the "Coordinates type" line (OrdinaryKriging, ok.py:333)
+    _KIND = None
+    _universal = False
+    _k_before_points = False
+    _prints_coordinates_type = False
 
     # ---- variogram model selection (ok.py:208-253; GSTools models arrive as 'custom') ----
-    def _select_variogram(self, variogram_model, variogram_function, gstools_dim_ok):
+    def _select_variogram(self, variogram_model, variogram_function, variogram_parameters, anisotropy, check_latlon):
+        """Returns the (variogram_parameters, anisotropy) that apply: a GSTools CovModel brings its own callable and
+        anisotropy (ok.py:224-239)."""
         self.variogram_model = variogram_model
         self.model = None
-        overrides = {}
         if hasattr(self.variogram_model, "pykrige_kwargs"):
+            from .compat_gstools import validate_gstools
+
             self.model = self.variogram_model
-            gstools_dim_ok(self.model)
+            validate_gstools(self.model)
+            if self._ndim == 2 and self.model.field_dim == 3:
+                raise ValueError("GSTools: model dim is not 1 or 2")
+            if self._ndim == 3 and self.model.field_dim < 3:
+                raise ValueError("GSTools: model dim is not 3")
+            if check_latlon and self.model.latlon and self.coordinates_type == "euclidean":
+                raise ValueError("GSTools: latlon models require geographic coordinates")
             self.variogram_model = "custom"
             variogram_function = self.model.pykrige_vario
-            overrides["variogram_parameters"] = []
-            overrides["gstools"] = self.model
+            variogram_parameters = []
+            anisotropy = tuple(getattr(self.model, a.replace("anisotropy_scaling", "pykrige_anis")
+                                       .replace("anisotropy_angle", "pykrige_angle"))
+                               for a in self._SCALINGS + self._ANGLES)
         if self.variogram_model not in self.variogram_dict.keys() and self.variogram_model != "custom":
             raise ValueError("Specified variogram model '%s' is not supported." % variogram_model)
         elif self.variogram_model == "custom":
@@ -45,7 +82,7 @@ class KrigeBase:
             self.variogram_function = variogram_function
         else:
             self.variogram_function = self.variogram_dict[self.variogram_model]
-        return overrides
+        return variogram_parameters, anisotropy
 
     def _print_variogram(self):
         p = self.variogram_model_parameters
@@ -66,6 +103,112 @@ class KrigeBase:
             print("Full Sill:", p[0] + p[2])
             print("Range:", p[1])
             print("Nugget:", p[2], "\n")
+
+    # ---- constructor and update_variogram_model ------------------------------------------------------------------
+    def _init_model(self, coords, values, variogram_model, variogram_parameters, variogram_function, nlags, weight,
+                    anisotropy, verbose, enable_plotting, exact_values, pseudo_inv, pseudo_inv_type,
+                    coordinates_type="euclidean", statistics="lazy"):
+        """The constructor body: option checks, GSTools hand-over, float64 copies of the data, anisotropy of the data,
+        variogram initialisation, statistics policy. coords = (x, y[, z]); anisotropy = the values of the anisotropy
+        attributes in argument order. statistics: 'off' (OrdinaryKriging default), 'eager' (enable_statistics=True) or
+        'lazy' (the other classes: the reference computes them in the constructor, uk.py:380; here on first access)."""
+        self.pseudo_inv = bool(pseudo_inv)
+        self.pseudo_inv_type = str(pseudo_inv_type)
+        if self.pseudo_inv_type not in P_INV_TYPES:
+            raise ValueError("pseudo inv type not valid: " + str(pseudo_inv_type))
+        if not isinstance(exact_values, bool):
+            raise ValueError("exact_values has to be boolean True or False")
+        if coordinates_type not in ("euclidean", "geographic"):
+            raise ValueError("Only 'euclidean' and 'geographic' are valid values for coordinates-keyword.")
+        self.exact_values = exact_values
+        self.coordinates_type = coordinates_type
+        self.verbose = verbose
+        self.enable_plotting = enable_plotting
+        variogram_parameters, anisotropy = self._select_variogram(
+            variogram_model, variogram_function, variogram_parameters, anisotropy, check_latlon=self._ndim == 2)
+
+        # 1-D float64 copies of the inputs (ok.py:262-268)
+        copies = [np.atleast_1d(np.squeeze(np.array(a, copy=True, dtype=np.float64))) for a in tuple(coords) + (values,)]
+        for name, a in zip([c + "_ORIG" for c in self._AXES] + [self._VALUES], copies):
+            setattr(self, name, a)
+        if self.enable_plotting and self.verbose:
+            print("Plotting Enabled\n")
+
+        if coordinates_type == "geographic":
+            # lon/lat in degrees (2-D only); anisotropy is ambiguous on the sphere and ignored (ok.py:292-306)
+            if anisotropy[0] != 1.0:
+                warnings.warn(GEO_ANISOTROPY_WARNING, UserWarning)
+            self.XCENTER = self.YCENTER = 0.0
+            self.anisotropy_scaling, self.anisotropy_angle = 1.0, 0.0
+            self.X_ADJUSTED, self.Y_ADJUSTED = self.X_ORIG, self.Y_ORIG
+        else:
+            for c in self._AXES:
+                orig = getattr(self, c + "_ORIG")
+                setattr(self, c + "CENTER", (np.amax(orig) + np.amin(orig)) / 2.0)
+            self._set_anisotropy(anisotropy)
+
+        if self.verbose:
+            print("Initializing variogram model...")
+        self._fit_variogram(variogram_parameters, nlags, weight)
+        self._statistics_policy(statistics)
+
+    def _update_variogram_model(self, variogram_model, variogram_parameters, variogram_function, nlags, weight,
+                                anisotropy):
+        variogram_parameters, anisotropy = self._select_variogram(
+            variogram_model, variogram_function, variogram_parameters, anisotropy, check_latlon=False)
+        if self.coordinates_type == "geographic":
+            if anisotropy[0] != 1.0:
+                warnings.warn(GEO_ANISOTROPY_WARNING, UserWarning)
+        elif tuple(anisotropy) != tuple(getattr(self, a) for a in self._SCALINGS + self._ANGLES):
+            self._set_anisotropy(anisotropy)
+        if self.verbose:
+            print("Updating variogram mode...")
+        self._fit_variogram(variogram_parameters, nlags, weight)
+        self._statistics_policy("lazy")
+
+    def _set_anisotropy(self, anisotropy):
+        """Sets the anisotropy attributes and moves the data to the adjusted frame (X_ADJUSTED, ...)."""
+        if self.verbose:
+            print("Adjusting data for anisotropy...")
+        for name, v in zip(self._SCALINGS + self._ANGLES, anisotropy):
+            setattr(self, name, v)
+        adjusted = self._adjust(*[getattr(self, c + "_ORIG") for c in self._AXES])
+        for c, a in zip(self._AXES, adjusted):
+            setattr(self, c + "_ADJUSTED", a)
+
+    def _adjust(self, *coords):
+        """This object's anisotropy applied to points given as coordinate arrays in the original frame: the adjusted
+        coordinate arrays, stacked [ndim, n] (core.py:120-193)."""
+        center, scalings, angles = self._anisotropy()
+        return _adjust_for_anisotropy(np.vstack(coords).T, center, scalings, angles).T
+
+    def _anisotropy(self):
+        """(center, scalings, angles) as lists."""
+        return ([getattr(self, c + "CENTER") for c in self._AXES], [getattr(self, a) for a in self._SCALINGS],
+                [getattr(self, a) for a in self._ANGLES])
+
+    def _fit_variogram(self, variogram_parameters, nlags, weight):
+        X, values = self._stats_inputs()
+        vp = _make_variogram_parameter_list(self.variogram_model, variogram_parameters)
+        self.lags, self.semivariance, self.variogram_model_parameters = _initialize_variogram_model(
+            X, values, self.variogram_model, vp, self.variogram_function, nlags, weight, self.coordinates_type,
+            lazy=True)
+        if self.verbose:
+            if self._prints_coordinates_type:
+                print("Coordinates type: '%s'" % self.coordinates_type, "\n")
+            self._print_variogram()
+        if self.enable_plotting:
+            self.display_variogram_model()
+
+    def _stats_inputs(self):
+        """(adjusted data coordinates [n, ndim], values)"""
+        return np.vstack([getattr(self, c + "_ADJUSTED") for c in self._AXES]).T, getattr(self, self._VALUES)
+
+    def _data_arrays(self):
+        """(x, y, z|None, values, center, Mt) in ORIGINAL coordinates."""
+        center, scalings, angles = self._anisotropy()
+        x, y, z = [getattr(self, c + "_ORIG") for c in self._AXES] + [None] * (3 - self._ndim)
+        return x, y, z, getattr(self, self._VALUES), center, core.anisotropy_matrix(self._ndim, scalings, angles)
 
     # ---- experimental variogram: computed on first access when the parameters were given explicitly
     #      (the reference always runs the O(N^2) pdist in the constructor, core.py:432-436) -------------
@@ -90,9 +233,6 @@ class KrigeBase:
 
     # ---- cross-validation statistics: lazy (the reference runs this O(N^4) loop in the
     #      constructor of OK3D/UK/UK3D, ok3d.py:352, uk.py:380, uk3d.py:380; SURVEY F5) -----
-    def _stats_inputs(self):
-        raise NotImplementedError
-
     def _device_statistics(self):
         """delta, sigma, epsilon from the Cholesky factor of the device problem (kb200_statistics,
         csrc/variogram.cu: O(N) after the factorisation instead of the reference's N solves). Returns
@@ -102,7 +242,7 @@ class KrigeBase:
             return None                          # core._krige solves with lstsq under pseudo_inv (core.py:749-750)
         try:
             key = getattr(self, "_kb_key", None)
-            if key is not None and key[1] is False and key == self._problem_signature(key[0], False):
+            if key is not None and not key.knn and key == self._problem_key(key.dtype, False):
                 h = self._cuda_handle()           # the factor of the last global execute() is still there
             else:
                 h = self._ensure_problem("float64")
@@ -246,6 +386,13 @@ class KrigeBase:
             self._kb_table_dmax = need if have == 0.0 else max(need, 2.0 * have)
         return self._kb_table_dmax
 
+    def _cover_prediction_points(self, axes):
+        """A tabulated variogram must reach every data-prediction distance: extends its range to the box of the
+        prediction points, axes = [x, y(, z)] grid axes or point lists (the same on every rank of a sharded run)."""
+        nd = self._ndim
+        if self._device_model()[0] == self.TABLE_MODEL_ID and all(np.size(a) for a in axes[:nd]):
+            self._table_dmax([float(np.min(a)) for a in axes[:nd]], [float(np.max(a)) for a in axes[:nd]])
+
     def _variogram_table(self, dmax):
         """gamma at the sqrt-spaced nodes d_i = dmax (i/(n-1))^2, cached per (callable, parameters, dmax)."""
         key = (id(self.variogram_function), tuple(np.ravel(np.asarray(self.variogram_model_parameters, dtype=float))),
@@ -264,13 +411,13 @@ class KrigeBase:
         self._kb_table = (key, g)
         return g
 
-    def _data_arrays(self):
-        """(x, y, z|None, values, center, Mt) in ORIGINAL coordinates."""
-        raise NotImplementedError
-
     def _drift_spec(self):
         """(n_rl, [host drift data columns])"""
         return 0, []
+
+    def _device_drift(self):
+        """(wells, ext) of the drift terms evaluated on the device (UniversalKriging: point_log, external_Z)."""
+        return None, None
 
     def _cuda_handle(self, n_gpus=None):
         """The C-ABI executor of this model: one kb200 handle (default) or, for n_gpus > 1, a kb200_group of
@@ -291,85 +438,65 @@ class KrigeBase:
             self._kb_key = None
         return h
 
-    def _content_digest(self):
-        """Cheap content hash of everything the device problem is built from (coordinates, values, host drift
-        columns), so that in-place edits of the data arrays invalidate the cached factorisation."""
-        import hashlib
-        x, y, z, v, center, Mt = self._data_arrays()
-        n_rl, cols = self._drift_spec()
-        hsh = hashlib.blake2b(digest_size=16)
-        for a in (x, y, z, v) + tuple(cols):
-            if a is not None:
-                hsh.update(np.ascontiguousarray(a, dtype=np.float64).tobytes())
-        return hsh.hexdigest()
-
-    def _problem_signature(self, dtype, knn, fields=None):
+    def _problem_key(self, dtype, knn, fields=None):
         x, y, z, v, center, Mt = self._data_arrays()
         mid, vp = self._device_model()
         n_rl, cols = self._drift_spec()
         if mid == self.TABLE_MODEL_ID:      # the table itself is part of the problem
             vp = ("table", id(self.variogram_function), getattr(self, "_kb_table_dmax", 0.0)) + tuple(
                 np.ravel(np.asarray(self.variogram_model_parameters, dtype=float)))
-        return (dtype, knn, mid, tuple(vp), bool(self.exact_values), tuple(np.ravel(Mt)), tuple(center),
-                n_rl, len(cols), x.size, getattr(self, "coordinates_type", "euclidean"),
-                bool(getattr(self, "pseudo_inv", False)), self._device_drift_signature(), self._content_digest(),
-                self._fields_signature(fields))
-
-    @staticmethod
-    def _fields_signature(fields):
-        """(V, digest) of the value fields a problem kriges instead of the constructor's values; (0, None) without."""
-        if fields is None:
-            return 0, None
-        import hashlib
-        return fields.shape[0], hashlib.blake2b(np.ascontiguousarray(fields).tobytes(), digest_size=16).hexdigest()
-
-    def _device_drift_signature(self):
-        return ()
-
-    def _configure_device_drift(self, h):
-        """Hook for drift terms evaluated on the device (UniversalKriging: point_log, external_Z)."""
-        h.set_device_drift(None, None)
+        wells, ext = self._device_drift()
+        hsh = hashlib.blake2b(digest_size=16)
+        for a in [x, y, z, v] + list(cols) + [wells] + list(ext or (None,)) + [fields]:
+            if a is None:
+                hsh.update(b"-")
+            else:
+                a = np.ascontiguousarray(a, dtype=np.float64)
+                hsh.update(repr(a.shape).encode())
+                hsh.update(a.tobytes())
+        return ProblemKey(dtype, knn, mid, tuple(vp), bool(self.exact_values), tuple(np.ravel(Mt)), tuple(center), n_rl,
+                          getattr(self, "coordinates_type", "euclidean") == "geographic",
+                          bool(getattr(self, "pseudo_inv", False)), 0 if fields is None else fields.shape[0],
+                          hsh.hexdigest())
 
     def _ensure_problem(self, dtype="float64", knn=False, n_gpus=None, fields=None):
-        name = dtype if isinstance(dtype, str) and dtype in _cabi.DTYPES else str(np.dtype(dtype))
-        dt = _cabi.DTYPES.get(name)
-        if dt is None:
-            raise ValueError("dtype must be one of %s" % ", ".join(repr(k) for k in _cabi.DTYPES))
+        dt = _cabi.dtype_code(dtype)
         h = self._cuda_handle(n_gpus)
-        grouped = isinstance(h, _cabi.Group)
+        slot = "_kb_gkey" if isinstance(h, _cabi.Group) else "_kb_key"
         if self._device_model()[0] == self.TABLE_MODEL_ID:
-            self._table_dmax()                  # fixes the tabulated range before it enters the signature
-        key = self._problem_signature(dt, knn, fields)
-        if (self._kb_gkey if grouped else self._kb_key) == key:
+            self._table_dmax()                  # fixes the tabulated range before it enters the key
+        key = self._problem_key(dt, knn, fields)
+        if getattr(self, slot) == key:
             return h
+        setattr(self, slot, None)
+        self._set_up_problem(h, dt, knn, fields)
+        setattr(self, slot, key)
+        return h
+
+    def _set_up_problem(self, h, dt, knn=False, fields=None, describe_only=False):
+        """Configures handle (or group) h for this object's problem, then hands the problem over: kb200_set_problem
+        (assemble and factor), kb200_set_problem_knn (the moving window) or, with describe_only, kb200_describe_problem
+        (record it and allocate the factor blob that a broadcast fills, multigpu.prepare_sharded)."""
         x, y, z, v, center, Mt = self._data_arrays()
         mid, vp = self._device_model()
-        n_rl, cols = self._drift_spec()
-        if grouped:
-            self._kb_gkey = None
-        else:
-            self._kb_key = None
         if knn and bool(getattr(self, "pseudo_inv", False)):
             warnings.warn("pseudo_inv is ignored by the moving window (n_closest_points), as in the reference "
                           "(ok.py:753 always calls scipy.linalg.solve).", UserWarning)
         h.set_coordinates(getattr(self, "coordinates_type", "euclidean") == "geographic")
         h.set_pseudo_inverse(bool(getattr(self, "pseudo_inv", False)) and not knn)
-        if mid == self.TABLE_MODEL_ID:
+        if mid == self.TABLE_MODEL_ID:          # 'custom' callable: every rank of a sharded run tabulates it itself
             dmax = self._table_dmax()
             h.set_variogram_table(self._variogram_table(dmax), dmax)
         if fields is not None or getattr(h, "n_fields", 0):
             h.set_values(fields)
         if knn:
             h.set_problem_knn(self._ndim, x, y, z, v, center, Mt, mid, vp, self.exact_values, self.eps)
-        else:
-            self._configure_device_drift(h)
-            h.set_problem(self._ndim, dt, x, y, z, v, center, Mt, mid, vp, self.exact_values, self.eps,
-                          n_rl=n_rl, drift_data=cols if cols else None)
-        if grouped:
-            self._kb_gkey = key
-        else:
-            self._kb_key = key
-        return h
+            return
+        h.set_device_drift(*self._device_drift())
+        n_rl, cols = self._drift_spec()
+        hand_over = h.describe_problem if describe_only else h.set_problem
+        hand_over(self._ndim, dt, x, y, z, v, center, Mt, mid, vp, self.exact_values, self.eps, n_rl=n_rl,
+                  drift_data=cols if cols else None)
 
     # ---- execute(): argument handling shared by the four classes ---------------------------------
     _MASK_DIM_MSG = {2: "Mask is not two-dimensional.", 3: "Mask is not three-dimensional."}
@@ -378,14 +505,23 @@ class KrigeBase:
         3: "xpoints, ypoints, and zpoints must have same dimensions when treated as listing discrete points.",
     }
 
+    @staticmethod
+    def _check_style(style):
+        if style != "grid" and style != "masked" and style != "points":
+            raise ValueError("style argument must be 'grid', 'points', or 'masked'")
+
+    @staticmethod
+    def _check_n_closest_points(n_closest_points):
+        if n_closest_points is not None and n_closest_points <= 1:
+            raise ValueError("n_closest_points has to be at least two!")
+
     def _prepare_points(self, style, coords, mask):
         """style / mask / point-list validation of execute() (ok.py:834-874, uk.py:1169-1215, ok3d.py:833-876,
         uk3d.py:981-1024), once for 2-D and 3-D. coords = (xpoints, ypoints[, zpoints]).
         Returns (axes: list of 1-D float64 arrays, sizes (nx, ny[, nz]), flat_mask or None); the mask is
         returned in the reference's flattened order (x fastest; 3-D: (z, y, x))."""
         nd = self._ndim
-        if style != "grid" and style != "masked" and style != "points":
-            raise ValueError("style argument must be 'grid', 'points', or 'masked'")
+        self._check_style(style)
         axes = [np.atleast_1d(np.squeeze(np.array(c, copy=True))) for c in coords]
         sizes = tuple(a.size for a in axes)
         flat_mask = None
@@ -407,7 +543,7 @@ class KrigeBase:
                 raise ValueError(self._POINTS_MSG[nd])
         return [a.astype(np.float64) for a in axes], sizes, flat_mask
 
-    def _specified_drift_grids(self, style, specified_drift_arrays, sizes, npoints, cls_name):
+    def _specified_drift_grids(self, style, specified_drift_arrays, sizes, npoints):
         """'specified' drift arrays at the prediction points: validation of uk.py:1217-1274 / uk3d.py:1040-1098.
         Returns the list of arrays in the reference's orientation ((ny, nx) / (nz, ny, nx) or (n,))."""
         nd = self._ndim
@@ -443,9 +579,12 @@ class KrigeBase:
         elif len(specified_drift_arrays) != 0:
             warnings.warn(
                 "Provided specified drift values, but 'specified' drift was not initialized during "
-                "instantiation of %s class." % cls_name, RuntimeWarning,
+                "instantiation of %s class." % ("UniversalKriging" if nd == 2 else "UniversalKriging3D"), RuntimeWarning,
             )
         return grids
+
+    def _check_drift_domain(self, axes):
+        """Hook: UniversalKriging checks that its external-Z raster covers the prediction points."""
 
     @staticmethod
     def _shape_output(style, z, ss, sizes, flat_mask):
@@ -460,12 +599,78 @@ class KrigeBase:
             ss = ss.reshape(sizes[::-1])
         return z, ss
 
-    # ---- execute(values=...): several value fields through one factorisation ---------------------------------
-    @staticmethod
-    def _fields_kw(fields):
-        """Keyword for _run_cuda: without fields the call is the single-field call, unchanged."""
-        return {} if fields is None else {"fields": fields}
+    def _execute(self, style, coords, mask, backend, n_closest_points=None, specified_drift_arrays=None,
+                 dtype="float64", n_gpus=None, values=None):
+        """The body of the four execute() methods, each class's checks in the order the reference makes them."""
+        if self.verbose:
+            print("Executing %s Kriging...\n" % ("Universal" if self._universal else "Ordinary"))
+        if self._k_before_points:
+            self._check_style(style)
+            self._check_n_closest_points(n_closest_points)
+        axes, sizes, flat_mask = self._prepare_points(style, coords, mask)
+        self._check_n_closest_points(n_closest_points)
+        drift_at = None
+        if self._universal:
+            drift_at = self._host_drift_at(self._specified_drift_grids(style, specified_drift_arrays, sizes,
+                                                                       axes[0].size))
+        self._check_backend(backend, self._KIND)
+        self._check_drift_domain(axes)
+        fields, one = self._check_values(values, dtype, n_closest_points, n_gpus)
+        z, ss = self._run_cuda(style, axes, flat_mask, n_closest_points=n_closest_points, drift_at=drift_at,
+                               dtype=dtype, n_gpus=n_gpus, fields=fields)
+        return self._shape_output(style, z[0] if one else z, ss, sizes, flat_mask)
 
+    # ---- 'specified' and 'functional' drift terms of the universal classes ---------------------------------------
+    def _init_host_drift_terms(self, drift_terms, specified_drift, functional_drift):
+        """The 'specified' (uk.py:476-494) and 'functional' (uk.py:496-510) drift terms of the constructor."""
+        if specified_drift is None:
+            specified_drift = []
+        if functional_drift is None:
+            functional_drift = []
+        if "specified" in drift_terms:
+            if type(specified_drift) is not list:
+                raise TypeError("Arrays for specified drift terms must be encapsulated in a list.")
+            if len(specified_drift) == 0:
+                raise ValueError("Must provide at least one drift-value array when using the 'specified' drift capability.")
+            self.specified_drift = True
+            self.specified_drift_data_arrays = []
+            for term in specified_drift:
+                specified = np.squeeze(np.array(term, copy=True))
+                if specified.size != self.X_ORIG.size:
+                    raise ValueError("Must specify the drift values for each data point when using the 'specified' drift capability.")
+                self.specified_drift_data_arrays.append(specified)
+        else:
+            self.specified_drift = False
+        # functional drift: callables evaluated with the adjusted coordinates
+        if "functional" in drift_terms:
+            if type(functional_drift) is not list:
+                raise TypeError("Callables for functional drift terms must be encapsulated in a list.")
+            if len(functional_drift) == 0:
+                raise ValueError("Must provide at least one callable object when using the 'functional' drift capability.")
+            self.functional_drift = True
+            self.functional_drift_terms = functional_drift
+        else:
+            self.functional_drift = False
+
+    def _host_drift_at(self, spec_drift_grids):
+        """The drift_at callback of a run (see _run_cuda): the 'specified' and 'functional' drift values at the
+        prediction points (uk.py:972-979, uk3d.py:1100-1110), or None without such terms."""
+        if not (self.specified_drift or self.functional_drift):
+            return None
+
+        def drift_at(pts, idx):
+            cols = []
+            for g in spec_drift_grids:
+                flat = np.asarray(g, dtype=float).flatten()
+                cols.append(flat if idx is None else flat[idx])
+            if self.functional_drift:
+                adjusted = self._adjust(*pts)
+                for func in self.functional_drift_terms:
+                    cols.append(np.asarray(func(*adjusted), dtype=float) * np.ones(adjusted[0].shape))
+            return np.ascontiguousarray(np.vstack(cols), dtype=np.float64)
+        return drift_at
+
+    # ---- execute(values=...): several value fields through one factorisation ---------------------------------
     def _check_values(self, values, dtype, n_closest_points, n_gpus):
         """Validates the values= keyword of execute() after the reference's own argument checks. Returns
         (fields as a (V, N) float64 array, whether values was 1-D), or (None, False) for values=None."""
@@ -484,14 +689,27 @@ class KrigeBase:
             raise ValueError("values has no fields (V = 0)")
         if not np.all(np.isfinite(v)):
             raise ValueError("values must be finite")
-        name = dtype if isinstance(dtype, str) else str(np.dtype(dtype))
-        if name != "float64":
+        if _cabi.dtype_name(dtype) != "float64":
             raise NotImplementedError("execute(values=...) runs in dtype='float64' only")
         if bool(getattr(self, "pseudo_inv", False)) and n_closest_points is None:
             raise NotImplementedError("execute(values=...) is not supported with pseudo_inv=True")
         if n_gpus is not None and int(n_gpus) > 1:
             raise NotImplementedError("execute(values=...) runs on one GPU (n_gpus > 1 is not supported)")
         return np.ascontiguousarray(v.T), one
+
+    @staticmethod
+    def _per_chunk(fields, run):
+        """run(chunk) -> (z, ss) once with chunk None (no fields) or once per chunk of at most _cabi.MAX_FIELDS
+        fields, each its own problem (factorisation); z then is (V, m): every field's result is independent of the
+        chunk it is in."""
+        if fields is None:
+            return run(None)
+        zs = []
+        for c0 in range(0, fields.shape[0], _cabi.MAX_FIELDS):
+            chunk = fields[c0:c0 + _cabi.MAX_FIELDS]
+            z, ss = run(chunk)
+            zs.append(np.reshape(z, (chunk.shape[0], -1)))
+        return np.concatenate(zs), ss
 
     # ---- the device run: plan (what to compute) -> run (one contiguous block of it) -> scatter ----
     def _plan(self, style, axes, mask, drift_at=None):
@@ -553,35 +771,25 @@ class KrigeBase:
         host-supplied drift values at the given points, or None.  n_gpus: None/1 = this handle's device;
         G > 1 = single-process multi-GPU (one host thread, kb200_group_*: device 0 factors, peer copies of the
         factor blob, contiguous blocks of the work list, results gathered in the reference's order).
-        fields: (V, N) value fields kriged instead of the constructor's values, or None.
-        Returns flat (z, ss) of length npt in the reference's flattened order; z is (V, npt) with fields.
-        More than _cabi.MAX_FIELDS fields run as chunks of that many, each its own problem (factorisation) and
-        execute; every field's result is independent of the chunk it is in."""
+        fields: (V, N) value fields kriged instead of the constructor's values, or None (see _per_chunk).
+        Returns flat (z, ss) of length npt in the reference's flattened order; z is (V, npt) with fields."""
         knn = n_closest_points is not None
-        nd = self._ndim
-        if self._device_model()[0] == self.TABLE_MODEL_ID and all(np.size(a) for a in axes[:nd]):
-            self._table_dmax([float(np.min(a)) for a in axes[:nd]], [float(np.max(a)) for a in axes[:nd]])
-        if fields is None:
-            h = self._ensure_problem(dtype, knn, n_gpus=n_gpus)
-            plan = self._plan(style, axes, mask, drift_at)
-            z, ss = self._run_block(h, plan, 0, plan["count"], n_closest_points, drift_at)
-            return self._scatter(plan, z, ss)
+        self._cover_prediction_points(axes)
         plan = self._plan(style, axes, mask, drift_at)
-        zs = []
-        for c0 in range(0, fields.shape[0], _cabi.MAX_FIELDS):
-            chunk = fields[c0:c0 + _cabi.MAX_FIELDS]
+
+        def run(chunk):
             h = self._ensure_problem(dtype, knn, n_gpus=n_gpus, fields=chunk)
-            z, ss = self._run_block(h, plan, 0, plan["count"], n_closest_points, drift_at)
-            zs.append(np.reshape(z, (chunk.shape[0], -1)))
-        return self._scatter(plan, np.concatenate(zs), ss)
+            return self._run_block(h, plan, 0, plan["count"], n_closest_points, drift_at)
+        z, ss = self._per_chunk(fields, run)
+        return self._scatter(plan, z, ss)
 
     # ---- leave_one_out(): cross-validation of every station --------------------------------------------------
-    def _leave_one_out(self, n_closest_points, values, backend, what):
+    def _leave_one_out(self, n_closest_points, values, backend):
         """(zvalues, sigmasq) of kriging every station from the other N - 1 with this object's fixed variogram
         (DESIGN.md §5e): the global path from the factorisation the last float64 execute() left on the handle (or a
         new one, which a later execute() reuses), the moving window with n_closest_points neighbours. values as in
         execute(values=...): zvalues is (V, N) for a 2-D values, (N,) otherwise; sigmasq is (N,)."""
-        self._check_backend(backend, what)
+        self._check_backend(backend, self._KIND)
         n = int(np.size(self._data_arrays()[3]))
         if n < 2:
             raise ValueError("leave-one-out needs at least two data points, got %d" % n)
@@ -594,16 +802,10 @@ class KrigeBase:
                                       "leave-one-out identities need the inverse of the kriging matrix")
         fields, one = self._check_values(values, "float64", n_closest_points, None)
 
-        def run(h):
+        def run(chunk):
+            h = self._ensure_problem("float64", knn, fields=chunk)
             return h.knn_loo(int(n_closest_points), n) if knn else h.loo(n)
-        if fields is None:
-            return run(self._ensure_problem("float64", knn))
-        zs = []
-        for c0 in range(0, fields.shape[0], _cabi.MAX_FIELDS):
-            chunk = fields[c0:c0 + _cabi.MAX_FIELDS]
-            z, ss = run(self._ensure_problem("float64", knn, fields=chunk))
-            zs.append(np.reshape(z, (chunk.shape[0], n)))
-        z = np.concatenate(zs)
+        z, ss = self._per_chunk(fields, run)
         return (z[0] if one else z), ss
 
     @staticmethod
@@ -613,3 +815,36 @@ class KrigeBase:
                 "Specified backend {} is not supported for {}: this package implements backend='cuda' only "
                 "(the reference's 'vectorized'/'loop'/'C' CPU paths live in PyKrige).".format(backend, what)
             )
+
+
+class Krige2D(KrigeBase):
+    """OrdinaryKriging and UniversalKriging: data X_ORIG, Y_ORIG with values Z; geographic coordinates exist here."""
+    _ndim = 2
+    _AXES = "XY"
+    _VALUES = "Z"
+    _SCALINGS = ("anisotropy_scaling",)
+    _ANGLES = ("anisotropy_angle",)
+
+    def update_variogram_model(self, variogram_model, variogram_parameters=None, variogram_function=None, nlags=6,
+                               weight=False, anisotropy_scaling=1.0, anisotropy_angle=0.0):
+        """Change the variogram model and/or its parameters (ok.py:379-553, uk.py:630-790). The statistics are
+        recomputed on their next access (the reference recomputes them here)."""
+        self._update_variogram_model(variogram_model, variogram_parameters, variogram_function, nlags, weight,
+                                     (anisotropy_scaling, anisotropy_angle))
+
+
+class Krige3D(KrigeBase):
+    """OrdinaryKriging3D and UniversalKriging3D: data X_ORIG, Y_ORIG, Z_ORIG with values VALUES."""
+    _ndim = 3
+    _AXES = "XYZ"
+    _VALUES = "VALUES"
+    _SCALINGS = ("anisotropy_scaling_y", "anisotropy_scaling_z")
+    _ANGLES = ("anisotropy_angle_x", "anisotropy_angle_y", "anisotropy_angle_z")
+
+    def update_variogram_model(self, variogram_model, variogram_parameters=None, variogram_function=None,
+                               nlags=6, weight=False, anisotropy_scaling_y=1.0, anisotropy_scaling_z=1.0,
+                               anisotropy_angle_x=0.0, anisotropy_angle_y=0.0, anisotropy_angle_z=0.0):
+        """Change the variogram model and/or its parameters (ok3d.py:354-520)."""
+        self._update_variogram_model(variogram_model, variogram_parameters, variogram_function, nlags, weight,
+                                     (anisotropy_scaling_y, anisotropy_scaling_z, anisotropy_angle_x,
+                                      anisotropy_angle_y, anisotropy_angle_z))

@@ -153,6 +153,19 @@ def device_available():
         return False
 
 
+def dtype_name(dtype):
+    """A key of DTYPES as given, otherwise numpy's name of the dtype ('f8' and np.float64 are 'float64')."""
+    return dtype if isinstance(dtype, str) and dtype in DTYPES else str(np.dtype(dtype))
+
+
+def dtype_code(dtype):
+    """The library's code (KB200_F64, ...) of a dtype; ValueError for one it does not have."""
+    code = DTYPES.get(dtype_name(dtype))
+    if code is None:
+        raise ValueError("dtype must be one of %s" % ", ".join(repr(k) for k in DTYPES))
+    return code
+
+
 def _ptr(a):
     return None if a is None else a.ctypes.data
 
@@ -165,44 +178,26 @@ TIMING_KEYS = ["assemble_ms", "cholesky_ms", "trtri_ms", "pack_dual_ms", "solve_
                "h2d_ms", "d2h_ms", "knn_search_ms", "knn_solve_ms", "solve_launches", "launches"]
 
 
-class Handle:
-    """Owns one kb200_handle. Error codes are mapped to the exception types the reference
-    raises at the same places (SURVEY.md §8b)."""
+class _Binding:
+    """What Handle and Group share: error codes mapped to the exception types the reference raises at the same places
+    (SURVEY.md §8b), and the marshalling of the problem and of the host execute calls, whose group entry points
+    (kb200_group_*) take the same arguments as the handle ones."""
 
     _PREFIX = "kb200_"
     _owned = True
     n_fields = 0        # value fields of the problem (kb200_set_values): z comes back as n_fields blocks
 
-    @classmethod
-    def _borrowed(cls, lib, raw):
-        """A view of a handle owned by someone else (a group member): never destroyed from here."""
-        self = cls.__new__(cls)
-        self.lib = lib
-        self._h = ctypes.c_void_p(raw)
-        self._owned = False
-        return self
-
-    def __init__(self, device=-1):
-        self.lib = load_library()
-        self._h = ctypes.c_void_p()
-        rc = self.lib.kb200_create(ctypes.byref(self._h), int(device))
-        if rc != KB200_OK:
-            self._h = None
-            raise KrigeB200Error(
-                "kb200_create failed (code %d): no usable CUDA device. backend='cuda' has no CPU fallback." % rc
-            )
-
     def close(self):
         if getattr(self, "_h", None):
             if self._owned:
-                self.lib.kb200_destroy(self._h)
+                self._fn("destroy")(self._h)
             self._h = None
 
     def _fn(self, name):
         return getattr(self.lib, self._PREFIX + name)
 
     def _errmsg(self):
-        msg = self.lib.kb200_last_error(self._h)
+        msg = self._fn("last_error")(self._h)
         return msg.decode() if msg else ""
 
     def __del__(self):
@@ -229,23 +224,26 @@ class Handle:
 
     # -- problem description ---------------------------------------------------------
     def _problem_args(self, dim, dtype, x, y, z, values, center, aniso, model, vparams, exact_values, eps,
-                      n_rl, drift_data):
+                      n_rl=0, drift_data=None, knn=False):
+        """The arguments of kb200_set_problem / kb200_describe_problem, or with knn those of kb200_set_problem_knn
+        (no dtype, no drift), and the arrays they point into, which must outlive the call."""
         x, y, values = _f64(x), _f64(y), _f64(values)
         z = _f64(z) if dim == 3 else None
         center = _f64(center)
         aniso = _f64(np.asarray(aniso).reshape(-1))
         vparams = _f64(vparams)
+        args = [int(x.size), _ptr(x), _ptr(y), _ptr(z), _ptr(values), _ptr(center), _ptr(aniso), int(model),
+                _ptr(vparams), int(vparams.size), int(bool(exact_values)), float(eps)]
+        keep = (x, y, z, values, center, aniso, vparams)
+        if knn:
+            return [self._h, int(dim)] + args, keep
         n_hd = 0
         if drift_data is not None and len(drift_data):
             drift_data = _f64(np.asarray(drift_data, dtype=np.float64).reshape(len(drift_data), -1))
             n_hd = drift_data.shape[0]
         else:
             drift_data = None
-        keep = (x, y, z, values, center, aniso, vparams, drift_data)
-        args = [self._h, int(dim), int(dtype), int(x.size), _ptr(x), _ptr(y), _ptr(z), _ptr(values),
-                _ptr(center), _ptr(aniso), int(model), _ptr(vparams), int(vparams.size),
-                int(bool(exact_values)), float(eps), int(n_rl), int(n_hd), _ptr(drift_data)]
-        return args, keep
+        return [self._h, int(dim), int(dtype)] + args + [int(n_rl), int(n_hd), _ptr(drift_data)], keep + (drift_data,)
 
     def set_problem(self, dim, dtype, x, y, z, values, center, aniso, model, vparams, exact_values, eps,
                     n_rl=0, drift_data=None):
@@ -253,28 +251,20 @@ class Handle:
                                         exact_values, eps, n_rl, drift_data)
         self._check(self._fn("set_problem")(*args))
 
-    def describe_problem(self, dim, dtype, x, y, z, values, center, aniso, model, vparams, exact_values, eps,
-                         n_rl=0, drift_data=None):
-        args, keep = self._problem_args(dim, dtype, x, y, z, values, center, aniso, model, vparams,
-                                        exact_values, eps, n_rl, drift_data)
-        self._check(self.lib.kb200_describe_problem(*args))
-
     def set_problem_knn(self, dim, x, y, z, values, center, aniso, model, vparams, exact_values, eps):
-        x, y, values = _f64(x), _f64(y), _f64(values)
-        z = _f64(z) if dim == 3 else None
-        center = _f64(center)
-        aniso = _f64(np.asarray(aniso).reshape(-1))
-        vparams = _f64(vparams)
-        self._check(self._fn("set_problem_knn")(
-            self._h, int(dim), int(x.size), _ptr(x), _ptr(y), _ptr(z), _ptr(values), _ptr(center), _ptr(aniso),
-            int(model), _ptr(vparams), int(vparams.size), int(bool(exact_values)), float(eps)))
+        args, keep = self._problem_args(dim, None, x, y, z, values, center, aniso, model, vparams, exact_values, eps,
+                                        knn=True)
+        self._check(self._fn("set_problem_knn")(*args))
 
     # -- execute (host buffers) --------------------------------------------------------
+    def _outputs(self, m):
+        """Host buffers of m results: z as max(1, n_fields) blocks of m, sigma^2 once."""
+        return np.empty(max(1, self.n_fields) * int(m), dtype=np.float64), np.empty(int(m), dtype=np.float64)
+
     def execute_points(self, px, py, pz=None, drift_pts=None):
         px, py, pz = _f64(px), _f64(py), _f64(pz)
         m = px.size
-        z = np.empty(max(1, self.n_fields) * m, dtype=np.float64)
-        ss = np.empty(m, dtype=np.float64)
+        z, ss = self._outputs(m)
         dpts = _f64(drift_pts)
         self._check(self._fn("execute_points")(self._h, m, _ptr(px), _ptr(py), _ptr(pz), _ptr(dpts),
                                                   _ptr(z), _ptr(ss)))
@@ -285,8 +275,7 @@ class Handle:
         nx, ny, nz = gx.size, gy.size, (gz.size if gz is not None else 1)
         if count is None:
             count = nx * ny * nz - first
-        z = np.empty(max(1, self.n_fields) * count, dtype=np.float64)
-        ss = np.empty(count, dtype=np.float64)
+        z, ss = self._outputs(count)
         dpts = _f64(drift_pts)
         self._check(self._fn("execute_grid")(self._h, nx, ny, nz, _ptr(gx), _ptr(gy), _ptr(gz), _ptr(dpts),
                                                 int(first), int(count), _ptr(z), _ptr(ss)))
@@ -295,8 +284,7 @@ class Handle:
     def execute_knn_points(self, k, px, py, pz=None):
         px, py, pz = _f64(px), _f64(py), _f64(pz)
         m = px.size
-        z = np.empty(max(1, self.n_fields) * m, dtype=np.float64)
-        ss = np.empty(m, dtype=np.float64)
+        z, ss = self._outputs(m)
         self._check(self._fn("execute_knn_points")(self._h, int(k), m, _ptr(px), _ptr(py), _ptr(pz),
                                                       _ptr(z), _ptr(ss)), knn=True)
         return z, ss
@@ -306,11 +294,39 @@ class Handle:
         nx, ny, nz = gx.size, gy.size, (gz.size if gz is not None else 1)
         if count is None:
             count = nx * ny * nz - first
-        z = np.empty(max(1, self.n_fields) * count, dtype=np.float64)
-        ss = np.empty(count, dtype=np.float64)
+        z, ss = self._outputs(count)
         self._check(self._fn("execute_knn_grid")(self._h, int(k), nx, ny, nz, _ptr(gx), _ptr(gy), _ptr(gz),
                                                     int(first), int(count), _ptr(z), _ptr(ss)), knn=True)
         return z, ss
+
+
+class Handle(_Binding):
+    """Owns one kb200_handle."""
+
+    @classmethod
+    def _borrowed(cls, lib, raw):
+        """A view of a handle owned by someone else (a group member): never destroyed from here."""
+        self = cls.__new__(cls)
+        self.lib = lib
+        self._h = ctypes.c_void_p(raw)
+        self._owned = False
+        return self
+
+    def __init__(self, device=-1):
+        self.lib = load_library()
+        self._h = ctypes.c_void_p()
+        rc = self.lib.kb200_create(ctypes.byref(self._h), int(device))
+        if rc != KB200_OK:
+            self._h = None
+            raise KrigeB200Error(
+                "kb200_create failed (code %d): no usable CUDA device. backend='cuda' has no CPU fallback." % rc
+            )
+
+    def describe_problem(self, dim, dtype, x, y, z, values, center, aniso, model, vparams, exact_values, eps,
+                         n_rl=0, drift_data=None):
+        args, keep = self._problem_args(dim, dtype, x, y, z, values, center, aniso, model, vparams,
+                                        exact_values, eps, n_rl, drift_data)
+        self._check(self.lib.kb200_describe_problem(*args))
 
     # -- execute (device pointers: raw addresses, e.g. torch_tensor.data_ptr()) -----------
     def execute_grid_dev(self, nx, ny, nz, d_gx, d_gy, d_gz, d_drift, first, count, d_z, d_ss):
@@ -390,7 +406,7 @@ class Handle:
         v = _f64(values)
         nl = int(nlags)
         cnt, sd, sg, mm = (np.zeros(max(nl, 0)), np.zeros(max(nl, 0)), np.zeros(max(nl, 0)), np.zeros(2))
-        self._check(self.lib.kb200_set_coordinates(self._h, 1 if geographic else 0))
+        self.set_coordinates(geographic)
         self._check(self.lib.kb200_experimental_variogram(
             self._h, dim, X.shape[0], _ptr(cols[0]), _ptr(cols[1]), _ptr(cols[2]) if dim > 2 else None,
             _ptr(v), nl, _ptr(cnt), _ptr(sd), _ptr(sg), _ptr(mm)))
@@ -407,15 +423,13 @@ class Handle:
     def loo(self, n):
         """Leave-one-out of every station of the problem kb200_set_problem factored on this handle (kb200_loo):
         (z, sigmasq), z as max(1, n_fields) blocks of the n stations."""
-        z = np.empty(max(1, self.n_fields) * int(n), dtype=np.float64)
-        ss = np.empty(int(n), dtype=np.float64)
+        z, ss = self._outputs(n)
         self._check(self.lib.kb200_loo(self._h, _ptr(z), _ptr(ss)))
         return z, ss
 
     def knn_loo(self, k, n):
         """Moving-window leave-one-out of every station with k neighbours from the other n - 1 (kb200_knn_loo)."""
-        z = np.empty(max(1, self.n_fields) * int(n), dtype=np.float64)
-        ss = np.empty(int(n), dtype=np.float64)
+        z, ss = self._outputs(n)
         self._check(self.lib.kb200_knn_loo(self._h, int(k), _ptr(z), _ptr(ss)), knn=True)
         return z, ss
 
@@ -427,9 +441,18 @@ class Handle:
         return out[:got]
 
 
-class Group(Handle):
-    """kb200_group: n_gpus handles behind one call from one host thread (single-process multi-GPU). Same
-    execute / set_problem methods as Handle; configuration calls fan out to the members."""
+def _on_every_member(name):
+    """A Group method that makes the same configuration call on every member handle."""
+    def call(self, *args):
+        for m in self.members:
+            getattr(m, name)(*args)
+    call.__name__ = name
+    return call
+
+
+class Group(_Binding):
+    """kb200_group: n_gpus handles behind one call from one host thread (single-process multi-GPU). The execute and
+    set_problem methods of Handle; configuration calls go to every member, the other calls of Handle it has not."""
 
     _PREFIX = "kb200_group_"
 
@@ -452,40 +475,17 @@ class Group(Handle):
         if getattr(self, "_h", None):
             for m in self.members:
                 m._h = None
-            self.lib.kb200_group_destroy(self._h)
-            self._h = None
+        super().close()
 
-    def _errmsg(self):
-        msg = self.lib.kb200_group_last_error(self._h)
-        return msg.decode() if msg else ""
-
-    def describe_problem(self, *a, **k):
-        raise NotImplementedError("a group factors on its first device and copies the blob itself")
-
-    # configuration: per member
-    def set_coordinates(self, geographic):
-        for m in self.members:
-            m.set_coordinates(geographic)
-
-    def set_pseudo_inverse(self, enable):
-        for m in self.members:
-            m.set_pseudo_inverse(enable)
-
-    def set_variogram_table(self, nodes, dmax):
-        for m in self.members:
-            m.set_variogram_table(nodes, dmax)
-
-    def set_device_drift(self, wells, ext):
-        for m in self.members:
-            m.set_device_drift(wells, ext)
+    set_coordinates = _on_every_member("set_coordinates")
+    set_pseudo_inverse = _on_every_member("set_pseudo_inverse")
+    set_variogram_table = _on_every_member("set_variogram_table")
+    set_device_drift = _on_every_member("set_device_drift")
+    reset_counters = _on_every_member("reset_counters")
 
     # instrumentation / constructor-side helpers: the factoring member
     def timings(self):
         return self.members[0].timings()
-
-    def reset_counters(self):
-        for m in self.members:
-            m.reset_counters()
 
     def statistics(self, n):
         return self.members[0].statistics(n)

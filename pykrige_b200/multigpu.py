@@ -14,6 +14,8 @@ The single-process variant (one host thread, ``execute(..., n_gpus=G)``) lives b
 """
 import numpy as np
 
+from . import _cabi
+
 
 def shard_range(count, rank, world):
     """Contiguous block [first, first+n) of `count` items for `rank` of `world` (sizes differ by <= 1)."""
@@ -45,30 +47,6 @@ def _active(dist):
     return dist is not None and dist.is_initialized() and dist.get_world_size() > 1
 
 
-def _dtype_code(dtype):
-    from . import _cabi
-    name = dtype if isinstance(dtype, str) and dtype in _cabi.DTYPES else str(np.dtype(dtype))
-    return _cabi.DTYPES[name]
-
-
-def _describe_only(model, dtype):
-    """Non-root rank: record the problem on the handle and allocate the blob, no device work."""
-    h = model._cuda_handle()
-    x, y, z, v, center, Mt = model._data_arrays()
-    mid, vp = model._device_model()
-    n_rl, cols = model._drift_spec()
-    h.set_coordinates(getattr(model, "coordinates_type", "euclidean") == "geographic")
-    h.set_pseudo_inverse(bool(getattr(model, "pseudo_inv", False)))
-    if mid == model.TABLE_MODEL_ID:      # 'custom' callable: every rank tabulates it itself (no broadcast)
-        dmax = model._table_dmax()
-        h.set_variogram_table(model._variogram_table(dmax), dmax)
-    model._configure_device_drift(h)
-    h.describe_problem(model._ndim, _dtype_code(dtype), x, y, z, v, center, Mt, mid, vp, model.exact_values,
-                       model.eps, n_rl=n_rl, drift_data=cols if cols else None)
-    model._kb_key = None
-    return h
-
-
 def prepare_sharded(model, dist=None, src=0, dtype="float64", device=None):
     """Make `model` ready to execute on every rank: rank `src` factors, everyone else only describes
     the problem (allocating the blob) and receives the broadcast. Returns the model's C-ABI handle.
@@ -89,8 +67,10 @@ def prepare_sharded(model, dist=None, src=0, dtype="float64", device=None):
             err = e
             status += 1
     else:
-        try:
-            h = _describe_only(model, dtype)
+        try:                              # record the problem and allocate the blob, no device work
+            h = model._cuda_handle()
+            model._kb_key = None
+            model._set_up_problem(h, _cabi.dtype_code(dtype), describe_only=True)
         except Exception as e:  # noqa: BLE001
             err = e
     dist.broadcast(status, src=src)      # one integer: did the factorisation succeed?
@@ -106,7 +86,7 @@ def prepare_sharded(model, dist=None, src=0, dtype="float64", device=None):
         torch.cuda.current_stream().synchronize()
     if rank != src:
         h.blob_commit()
-        model._kb_key = model._problem_signature(_dtype_code(dtype), False)
+        model._kb_key = model._problem_key(_cabi.dtype_code(dtype), False)
     return h
 
 
@@ -121,12 +101,8 @@ def execute_sharded(model, style, axes, dist=None, mask=None, n_closest_points=N
     Returns (z, ss, first, count): host arrays of the block and its position in the work list ('masked': the
     list of unmasked cells). With gather=True every rank returns the complete flat (z, ss) in the reference's
     order instead (all_gather_object; for tests and small jobs — the data path itself needs no gather)."""
-    knn = n_closest_points is not None
-    nd = model._ndim
-    if model._device_model()[0] == model.TABLE_MODEL_ID and all(np.size(a) for a in axes[:nd]):
-        # the tabulated range must cover the prediction points (same on every rank)
-        model._table_dmax([float(np.min(a)) for a in axes[:nd]], [float(np.max(a)) for a in axes[:nd]])
-    if knn:
+    model._cover_prediction_points(axes)
+    if n_closest_points is not None:
         h = model._ensure_problem("float64", knn=True)       # coordinates only: every rank builds its own cell grid
     else:
         h = prepare_sharded(model, dist, dtype=dtype, device=device)
@@ -146,9 +122,3 @@ def execute_sharded(model, style, axes, dist=None, mask=None, n_closest_points=N
         ss = np.concatenate([p[2] for p in parts])
     return model._scatter(plan, z, ss)
 
-
-def execute_grid_sharded(model, axes, dist=None, dtype="float64"):
-    """Krige this rank's contiguous slice of the flattened grid. Returns (z, ss, first, count) with host
-    arrays of the slice; concatenating the slices in rank order reproduces the single-GPU result bit
-    for bit (per-point arithmetic does not depend on the sharding)."""
-    return execute_sharded(model, "grid", axes, dist, dtype=dtype)

@@ -6,23 +6,24 @@ through libkrige_b200.so instead of scipy (no CPU fallback).
 """
 import numpy as np  # noqa: F401  (re-exported for callers that reach for ok.np like with the reference module)
 
-from ._base import KrigeBase
-from ._krige2d import Krige2DMixin, P_INV_TYPES  # noqa: F401
+from ._base import Krige2D, P_INV_TYPES  # noqa: F401
 
 
-class OrdinaryKriging(Krige2DMixin, KrigeBase):
+class OrdinaryKriging(Krige2D):
     """Two-dimensional ordinary kriging; see the reference docstring (ok.py:42-175) for the
     meaning of every argument. Only ``execute(..., backend='cuda')`` differs."""
+    _KIND = "2D ordinary kriging"
+    _k_before_points = True
     _prints_coordinates_type = True
 
     def __init__(self, x, y, z, variogram_model="linear", variogram_parameters=None, variogram_function=None, nlags=6,
                  weight=False, anisotropy_scaling=1.0, anisotropy_angle=0.0, verbose=False, enable_plotting=False,
                  enable_statistics=False, coordinates_type="euclidean", exact_values=True, pseudo_inv=False,
                  pseudo_inv_type="pinv"):
-        self._init_common_2d(x, y, z, variogram_model, variogram_parameters, variogram_function, nlags, weight,
-                             anisotropy_scaling, anisotropy_angle, verbose, enable_plotting, exact_values, pseudo_inv,
-                             pseudo_inv_type, coordinates_type=coordinates_type,
-                             statistics="eager" if enable_statistics else "off")
+        self._init_model((x, y), z, variogram_model, variogram_parameters, variogram_function, nlags, weight,
+                         (anisotropy_scaling, anisotropy_angle), verbose, enable_plotting, exact_values, pseudo_inv,
+                         pseudo_inv_type, coordinates_type=coordinates_type,
+                         statistics="eager" if enable_statistics else "off")
 
     def execute(self, style, xpoints, ypoints, mask=None, backend="cuda", n_closest_points=None, dtype="float64",
                 n_gpus=None, values=None):
@@ -42,20 +43,8 @@ class OrdinaryKriging(Krige2DMixin, KrigeBase):
         returns the usual shapes. float64 only, one GPU, not with ``pseudo_inv=True`` on the global path. Above
         ``KB200_MAX_FIELDS`` (64) fields the call runs in chunks of 64, each with its own factorisation.
         """
-        if self.verbose:
-            print("Executing Ordinary Kriging...\n")
-        if style != "grid" and style != "masked" and style != "points":
-            raise ValueError("style argument must be 'grid', 'points', or 'masked'")
-        if n_closest_points is not None and n_closest_points <= 1:
-            raise ValueError("n_closest_points has to be at least two!")
-        axes, sizes, flat_mask = self._prepare_points(style, (xpoints, ypoints), mask)
-        self._check_backend(backend, "2D ordinary kriging")
-        fields, one = self._check_values(values, dtype, n_closest_points, n_gpus)
-        zvalues, sigmasq = self._run_cuda(style, axes, flat_mask, n_closest_points=n_closest_points, dtype=dtype,
-                                          n_gpus=n_gpus, **self._fields_kw(fields))
-        if one:
-            zvalues = zvalues[0]
-        return self._shape_output(style, zvalues, sigmasq, sizes, flat_mask)
+        return self._execute(style, (xpoints, ypoints), mask, backend, n_closest_points=n_closest_points, dtype=dtype,
+                             n_gpus=n_gpus, values=values)
 
     def leave_one_out(self, n_closest_points=None, values=None, backend="cuda"):
         """Leave-one-out cross-validation: every station kriged from the other N - 1 stations with this object's fixed
@@ -69,4 +58,4 @@ class OrdinaryKriging(Krige2DMixin, KrigeBase):
         ``values`` (shape (N,) or (N, V)) as in execute(values=...). ``pseudo_inv=True`` is refused on the global path
         (NotImplementedError) and ignored by the moving window, as in execute().
         """
-        return self._leave_one_out(n_closest_points, values, backend, "2D ordinary kriging")
+        return self._leave_one_out(n_closest_points, values, backend)

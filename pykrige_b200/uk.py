@@ -8,9 +8,7 @@ kernels (kb200_set_device_drift), only specified / functional values (uk.py:972-
 """
 import numpy as np
 
-from ._base import KrigeBase
-from ._krige2d import Krige2DMixin, P_INV_TYPES  # noqa: F401
-from .core import _adjust_for_anisotropy
+from ._base import Krige2D, P_INV_TYPES  # noqa: F401
 
 
 def _first_last_index(axis, v):
@@ -24,10 +22,12 @@ def _first_last_index(axis, v):
     return i1, i2
 
 
-class UniversalKriging(Krige2DMixin, KrigeBase):
+class UniversalKriging(Krige2D):
     """Two-dimensional universal kriging; arguments as in the reference docstring (uk.py:40-205)."""
 
     UNBIAS = True  # the unbiasedness row is always present on the device path (uk.py:208)
+    _KIND = "2D universal kriging"
+    _universal = True
 
     def __init__(self, x, y, z, variogram_model="linear", variogram_parameters=None, variogram_function=None, nlags=6,
                  weight=False, anisotropy_scaling=1.0, anisotropy_angle=0.0, drift_terms=None, point_drift=None,
@@ -36,17 +36,13 @@ class UniversalKriging(Krige2DMixin, KrigeBase):
                  pseudo_inv_type="pinv"):
         if drift_terms is None:
             drift_terms = []
-        if specified_drift is None:
-            specified_drift = []
-        if functional_drift is None:
-            functional_drift = []
         # no drift term exists yet: the statistics the common body may compute (verbose=True) are those of the
         # ordinary-kriging system, as in the reference, where they precede the drift initialisation (uk.py:380-394)
         self.regional_linear_drift = self.external_Z_drift = self.point_log_drift = False
         self.specified_drift = self.functional_drift = False
-        self._init_common_2d(x, y, z, variogram_model, variogram_parameters, variogram_function, nlags, weight,
-                             anisotropy_scaling, anisotropy_angle, verbose, enable_plotting, exact_values, pseudo_inv,
-                             pseudo_inv_type, coordinates_type="euclidean", statistics="lazy")
+        self._init_model((x, y), z, variogram_model, variogram_parameters, variogram_function, nlags, weight,
+                         (anisotropy_scaling, anisotropy_angle), verbose, enable_plotting, exact_values, pseudo_inv,
+                         pseudo_inv_type)
 
         if self.verbose:
             print("Initializing drift terms...")
@@ -84,43 +80,14 @@ class UniversalKriging(Krige2DMixin, KrigeBase):
             point_log = np.atleast_2d(np.squeeze(np.array(point_drift, copy=True)))
             self.point_log_array = np.zeros(point_log.shape)
             self.point_log_array[:, 2] = point_log[:, 2]
-            self.point_log_array[:, :2] = _adjust_for_anisotropy(
-                np.vstack((point_log[:, 0], point_log[:, 1])).T,
-                [self.XCENTER, self.YCENTER],
-                [self.anisotropy_scaling],
-                [self.anisotropy_angle],
-            )
+            self.point_log_array[:, :2] = self._adjust(point_log[:, 0], point_log[:, 1]).T
             if self.verbose:
                 print("Implementing external point-logarithmic drift; number of points =",
                       self.point_log_array.shape[0], "\n")
         else:
             self.point_log_drift = False
 
-        if "specified" in drift_terms:
-            if type(specified_drift) is not list:
-                raise TypeError("Arrays for specified drift terms must be encapsulated in a list.")
-            if len(specified_drift) == 0:
-                raise ValueError("Must provide at least one drift-value array when using the 'specified' drift capability.")
-            self.specified_drift = True
-            self.specified_drift_data_arrays = []
-            for term in specified_drift:
-                specified = np.squeeze(np.array(term, copy=True))
-                if specified.size != self.X_ORIG.size:
-                    raise ValueError("Must specify the drift values for each data point when using the 'specified' drift capability.")
-                self.specified_drift_data_arrays.append(specified)
-        else:
-            self.specified_drift = False
-
-        # functional drift: callables evaluated with the adjusted coordinates (uk.py:496-510)
-        if "functional" in drift_terms:
-            if type(functional_drift) is not list:
-                raise TypeError("Callables for functional drift terms must be encapsulated in a list.")
-            if len(functional_drift) == 0:
-                raise ValueError("Must provide at least one callable object when using the 'functional' drift capability.")
-            self.functional_drift = True
-            self.functional_drift_terms = functional_drift
-        else:
-            self.functional_drift = False
+        self._init_host_drift_terms(drift_terms, specified_drift, functional_drift)
 
     def _calculate_data_point_zscalars(self, x, y, type_="array"):
         """Bilinear sample of the external-Z grid at (x, y) (uk.py:512-628), vectorised; node
@@ -177,23 +144,21 @@ class UniversalKriging(Krige2DMixin, KrigeBase):
                 cols.append(np.asarray(func(self.X_ADJUSTED, self.Y_ADJUSTED), dtype=float))
         return (2 if self.regional_linear_drift else 0), cols
 
-    def _device_drift_signature(self):
-        """point_log wells and the external-Z raster are evaluated at the prediction points by the solve
-        kernels themselves (kb200_set_device_drift); their content is part of the problem key."""
-        import hashlib
-        hsh = hashlib.blake2b(digest_size=16)
-        if self.point_log_drift:
-            hsh.update(np.ascontiguousarray(self.point_log_array, dtype=np.float64).tobytes())
-        if self.external_Z_drift:
-            for a in (self.external_Z_array_x, self.external_Z_array_y, self.external_Z_array):
-                hsh.update(np.ascontiguousarray(a, dtype=np.float64).tobytes())
-        return (bool(self.point_log_drift), bool(self.external_Z_drift), hsh.hexdigest())
-
-    def _configure_device_drift(self, h):
+    def _device_drift(self):
+        """point_log wells and the external-Z raster are evaluated at the prediction points by the solve kernels
+        themselves (kb200_set_device_drift)."""
         wells = self.point_log_array if self.point_log_drift else None
         ext = ((self.external_Z_array_x, self.external_Z_array_y, self.external_Z_array)
                if self.external_Z_drift else None)
-        h.set_device_drift(wells, ext)
+        return wells, ext
+
+    def _check_drift_domain(self, axes):
+        xpts, ypts = axes
+        if self.external_Z_drift and xpts.size and ypts.size:
+            ax, ay = self.external_Z_array_x, self.external_Z_array_y      # domain check of uk.py:545-551
+            if (np.amax(xpts) > np.amax(ax) or np.amin(xpts) < np.amin(ax)
+                    or np.amax(ypts) > np.amax(ay) or np.amin(ypts) < np.amin(ay)):
+                raise ValueError("External drift array does not cover specified kriging domain.")
 
     def execute(self, style, xpoints, ypoints, mask=None, backend="cuda", specified_drift_arrays=None,
                 dtype="float64", n_gpus=None, values=None):
@@ -210,41 +175,8 @@ class UniversalKriging(Krige2DMixin, KrigeBase):
         returns the usual shapes. float64 only, one GPU, not with ``pseudo_inv=True`` on the global path. Above
         ``KB200_MAX_FIELDS`` (64) fields the call runs in chunks of 64, each with its own factorisation.
         """
-        if self.verbose:
-            print("Executing Universal Kriging...\n")
-        axes, sizes, flat_mask = self._prepare_points(style, (xpoints, ypoints), mask)
-        xpts, ypts = axes
-        spec_drift_grids = self._specified_drift_grids(style, specified_drift_arrays, sizes, xpts.size,
-                                                       "UniversalKriging")
-        self._check_backend(backend, "2D universal kriging")
-        if self.external_Z_drift and xpts.size and ypts.size:
-            ax, ay = self.external_Z_array_x, self.external_Z_array_y      # domain check of uk.py:545-551
-            if (np.amax(xpts) > np.amax(ax) or np.amin(xpts) < np.amin(ax)
-                    or np.amax(ypts) > np.amax(ay) or np.amin(ypts) < np.amin(ay)):
-                raise ValueError("External drift array does not cover specified kriging domain.")
-
-        drift_at = None
-        if self.specified_drift or self.functional_drift:
-            def drift_at(pts, idx):
-                cols = []
-                if self.specified_drift:
-                    for g in spec_drift_grids:
-                        flat = np.asarray(g, dtype=float).flatten()
-                        cols.append(flat if idx is None else flat[idx])
-                if self.functional_drift:
-                    xa, ya = _adjust_for_anisotropy(
-                        np.vstack((pts[0], pts[1])).T, [self.XCENTER, self.YCENTER],
-                        [self.anisotropy_scaling], [self.anisotropy_angle]).T
-                    for func in self.functional_drift_terms:
-                        cols.append(np.asarray(func(xa, ya), dtype=float) * np.ones(xa.shape))
-                return np.ascontiguousarray(np.vstack(cols), dtype=np.float64)
-
-        fields, one = self._check_values(values, dtype, None, n_gpus)
-        zvalues, sigmasq = self._run_cuda(style, axes, flat_mask, drift_at=drift_at, dtype=dtype, n_gpus=n_gpus,
-                                          **self._fields_kw(fields))
-        if one:
-            zvalues = zvalues[0]
-        return self._shape_output(style, zvalues, sigmasq, sizes, flat_mask)
+        return self._execute(style, (xpoints, ypoints), mask, backend, specified_drift_arrays=specified_drift_arrays,
+                             dtype=dtype, n_gpus=n_gpus, values=values)
 
     def leave_one_out(self, values=None, backend="cuda"):
         """Leave-one-out cross-validation: every station kriged from the other N - 1 stations with this object's fixed
@@ -257,4 +189,4 @@ class UniversalKriging(Krige2DMixin, KrigeBase):
         execute(values=...). Raises ``numpy.linalg.LinAlgError`` naming the station when leaving it out leaves the
         drift terms undetermined, and NotImplementedError with ``pseudo_inv=True``.
         """
-        return self._leave_one_out(None, values, backend, "2D universal kriging")
+        return self._leave_one_out(None, values, backend)

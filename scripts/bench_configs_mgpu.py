@@ -64,7 +64,7 @@ def run_global(name, model, axes, dtype, group, nranks, flop_pt):
     npt = int(np.prod([a.size for a in axes]))
     def step():
         model._kb_key = None
-        return multigpu.execute_grid_sharded(model, axes, d, dtype=dtype)
+        return multigpu.execute_sharded(model, "grid", axes, d, dtype=dtype)
     step()                                   # warm-up (allocations, first factorisation)
     dt, (z, ss, first, count) = timed(step, group, nranks)
     emit({"config": name, "n_gpus": nranks, "dtype": dtype, "grid_points": npt, "seconds_max_over_ranks": dt,

@@ -141,6 +141,18 @@ def test_refusals(pk):
         ok.execute("points", *p, values=good, n_closest_points=1)
 
 
+def test_every_float64_spelling_is_accepted(pk):
+    """Every dtype spelling that execute() runs as float64 also runs with values=, with the same result."""
+    xyz, val = _data("ok")
+    coords = _grid_args("ok")
+    F = _fields(4, xyz.shape[0], 2)
+    z0, s0 = _make(pk, "ok", xyz, val).execute("grid", *coords, values=F)
+    for dtype in ("f8", np.float64, np.dtype("float64")):
+        z, s = _make(pk, "ok", xyz, val).execute("grid", *coords, values=F, dtype=dtype)
+        assert_array_equal(z, z0)
+        assert_array_equal(s, s0)
+
+
 def test_chunking_is_invisible(pk, monkeypatch):
     """Above the field limit the call runs as several problems; field v's result does not change."""
     from pykrige_b200 import _cabi
@@ -166,11 +178,11 @@ def test_cache_and_statistics_are_unchanged(pk):
     z0, s0 = ok.execute("grid", *coords)
     F = _fields(9, xyz.shape[0], 2)
     ok.execute("grid", *coords, values=F)
-    assert ok._kb_key[-1][0] == 2
+    assert ok._kb_key.n_fields == 2
     z1, s1 = ok.execute("grid", *coords)
     assert_array_equal(z1, z0)
     assert_array_equal(s1, s0)
-    assert ok._kb_key[-1] == (0, None)
+    assert ok._kb_key.n_fields == 0 and ok._kb_key == ok._problem_key(ok._kb_key.dtype, False)
     assert (ok.Q1, ok.Q2, ok.cR) == q
     np.testing.assert_array_equal(ok.Z, val)
     F2 = F.copy()

@@ -27,6 +27,19 @@ def test_library_exports_every_declared_symbol():
     assert lib.kb200_version() >= 1000
 
 
+def test_group_offers_only_what_a_group_can_serve():
+    """_cabi.Group shares the error mapping, the problem marshalling and the host execute calls with _cabi.Handle, but
+    not the handle-only calls: those would hand the group's pointer to kb200_* functions that expect a handle."""
+    for name in ("set_stream", "set_values", "blob_commit", "execute_grid_dev", "execute_points_dev",
+                 "execute_knn_grid_dev", "experimental_variogram", "loo", "knn_loo", "debug_fetch"):
+        assert hasattr(_cabi.Handle, name), name
+        assert not hasattr(_cabi.Group, name), name
+    for name in ("set_problem", "set_problem_knn", "execute_points", "execute_grid", "execute_knn_points",
+                 "execute_knn_grid", "set_coordinates", "set_pseudo_inverse", "set_variogram_table",
+                 "set_device_drift", "reset_counters", "timings", "statistics", "blob"):
+        assert hasattr(_cabi.Group, name), name
+
+
 def test_no_gpu_fails_loudly():
     import torch
     if torch.cuda.is_available():

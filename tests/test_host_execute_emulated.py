@@ -129,7 +129,7 @@ def test_reference_golden_grids_through_the_host_wrappers(pk, ref_goldens):
 
 def test_problem_cache_follows_the_data(pk):
     """execute() twice: the second call reuses the described problem; editing the data in place, changing the
-    variogram or switching the moving window on describes it again (_problem_signature / _content_digest)."""
+    variogram or switching the moving window on describes it again (_problem_key)."""
     xyz, val = cases.synth_data(321, 80, 2)
     m = pk.OrdinaryKriging(xyz[:, 0], xyz[:, 1], val, variogram_model="exponential", variogram_parameters=[1.0, 300.0, 0.05])
     gx = gy = np.linspace(0.0, 1000.0, 9)

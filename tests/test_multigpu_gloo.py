@@ -202,6 +202,9 @@ def _emulated_jobs():
     spec_pts = 1.0e-5 * px * py
     jobs = [
         ("uk_grid", "UniversalKriging", (xyz[:, 0], xyz[:, 1], val), uk_kw, ("grid", gx, gy), dict(specified_drift_arrays=[spec_grid])),
+        # execute(values=...) first: its value fields must not stay on the handle of the rank that only describes
+        ("uk_grid_after_fields", "UniversalKriging", (xyz[:, 0], xyz[:, 1], val), uk_kw, ("grid", gx, gy),
+         dict(specified_drift_arrays=[spec_grid])),
         ("uk_masked", "UniversalKriging", (xyz[:, 0], xyz[:, 1], val), uk_kw, ("masked", gx, gy), dict(mask=mask, specified_drift_arrays=[spec_grid])),
         ("uk_points", "UniversalKriging", (xyz[:, 0], xyz[:, 1], val), uk_kw, ("points", px, py), dict(specified_drift_arrays=[spec_pts])),
         ("ok3d_masked", "OrdinaryKriging3D", (x3[:, 0], x3[:, 1], x3[:, 2], v3), vp, ("masked", gx, gy, gz), dict(mask=mask3)),
@@ -218,7 +221,8 @@ def _emulated_jobs():
 def _sharded_execute(model, multigpu, dist, args, kw, device):
     """What a caller of execute() does under torchrun: the class validates and plans, execute_sharded runs the block.
     Uses the public execute() with `_run_cuda` re-routed to the sharded executor (gather=True)."""
-    def run_cuda(style, axes, mask, n_closest_points=None, drift_at=None, dtype="float64", n_gpus=None):
+    def run_cuda(style, axes, mask, n_closest_points=None, drift_at=None, dtype="float64", n_gpus=None, fields=None):
+        assert fields is None
         return multigpu.execute_sharded(model, style, axes, dist, mask=mask, n_closest_points=n_closest_points,
                                         dtype=dtype, drift_at=drift_at, gather=True, device=device)
     model._run_cuda = run_cuda
@@ -233,18 +237,22 @@ def _worker_emulated(rank, world, port, outdir):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     import pykrige_b200 as pk
     from pykrige_b200 import multigpu, _cabi
-    from abi_emulator import EmulatedHandle
+    from fields_emulator import FieldsEmulatedHandle
 
     def no_device():
         raise _cabi.KrigeB200Error("emulated box")
 
-    _cabi.Handle = EmulatedHandle
+    _cabi.Handle = FieldsEmulatedHandle
     _cabi.aux_handle = no_device
     multigpu.blob_as_tensor = lambda h, device: h.blob_t
     cpu = torch.device("cpu")
     out = {}
     for name, cls, cargs, ckw, eargs, ekw in _emulated_jobs():
         m = getattr(pk, cls)(*cargs, **ckw)
+        if name.endswith("_after_fields"):
+            v = cargs[-1]
+            m.execute(*eargs, backend="cuda", values=np.column_stack([v, v[::-1]]), **ekw)
+            del m._kb_handle.calls[:]
         z, ss = _sharded_execute(m, multigpu, dist, eargs, ekw, cpu)
         out[name + "_z"], out[name + "_ss"] = np.ma.getdata(z), np.ma.getdata(ss)
         out[name + "_calls"] = np.array(",".join(m._kb_handle.calls))
@@ -255,7 +263,8 @@ def _worker_emulated(rank, world, port, outdir):
 
 def test_two_rank_sharding_of_every_problem_kind(tmp_path, monkeypatch):
     """2 gloo ranks vs one process, both through the C-ABI emulator: universal kriging with all five drift kinds
-    (grid / masked / points — the host drift callback must be evaluated at the block's own positions), 3-D masked,
+    (grid / masked / points — the host drift callback must be evaluated at the block's own positions; also after an
+    execute(values=...) on the same objects), 3-D masked,
     UK3D points, the moving window (no broadcast) and a tabulated custom variogram (every rank tabulates itself)."""
     world = 2
     port = _free_port()
@@ -263,12 +272,12 @@ def test_two_rank_sharding_of_every_problem_kind(tmp_path, monkeypatch):
     sys.path.insert(0, os.path.join(ROOT, "tests"))
     import pykrige_b200 as pk
     from pykrige_b200 import _cabi
-    from abi_emulator import EmulatedHandle
+    from fields_emulator import FieldsEmulatedHandle
 
     def no_device():
         raise _cabi.KrigeB200Error("emulated box")
 
-    monkeypatch.setattr(_cabi, "Handle", EmulatedHandle)
+    monkeypatch.setattr(_cabi, "Handle", FieldsEmulatedHandle)
     monkeypatch.setattr(_cabi, "aux_handle", no_device)
     parts = [np.load(os.path.join(str(tmp_path), "e%d.npz" % r)) for r in range(world)]
     for name, cls, cargs, ckw, eargs, ekw in _emulated_jobs():
@@ -285,3 +294,5 @@ def test_two_rank_sharding_of_every_problem_kind(tmp_path, monkeypatch):
         else:                                                # rank 0 factors, rank 1 describes + commits the broadcast
             assert "set_problem" in c0.split(",") and "describe_problem" not in c0
             assert "describe_problem" in c1 and "blob_commit" in c1 and "set_problem" not in c1.split(",")
+        if name.endswith("_after_fields"):                   # the fields of the earlier run are dropped first
+            assert c1.split(",")[0] == "set_values"
