@@ -370,12 +370,33 @@ int kb200_statistics(kb200_handle h, double* delta, double* sigma);
 int kb200_loo(kb200_handle h, double* z, double* sigmasq);
 int kb200_knn_loo(kb200_handle h, int k, double* z, double* sigmasq);
 
+/* Leave-group-out cross-validation (DESIGN.md §5f): every station is kriged from the stations OUTSIDE its group, with
+ * the same fixed variogram, anisotropy, coordinate type, exact_values and drift terms. group[i] in [0, n_groups) is
+ * station i's group; n_groups >= 2 and no group is empty (else KB200_EBADARG). Outputs as kb200_loo.
+ *
+ * kb200_lgo runs after kb200_set_problem on THIS handle, from the factorisation it holds: G = C^-1 = W^T W once
+ * (O(n^3 / 3) on the DMMA pipe; the indefinite fallback already holds it), then per group S the block P_SS of
+ * P = C^-1 - U S^-1 U^T is inverted (in shared memory up to 128 stations, else by the blocked factor kernels), and
+ * zhat_S = Z_S - P_SS^-1 alpha_S, sigmasq_S = diag(P_SS^-1). When every group is a single station it runs kb200_loo
+ * (same bits, no O(n^3) step). A problem set with dtype KB200_F32 or KB200_F64X* is evaluated from the fp64 factor.
+ * Errors as kb200_loo: KB200_ESTATE, KB200_EUNSUPPORTED for the pseudo-inverse or more than 32 stations of other
+ * groups within eps of one station under exact_values, and KB200_ESINGULAR when leaving a group out leaves the drift
+ * terms undetermined (the message names the lowest such group and its lowest station).
+ *
+ * kb200_knn_lgo runs after kb200_set_problem_knn: the moving window with k neighbours taken from the stations outside
+ * the query station's group (ties by (d^2, original index)). 2 <= k <= n - (size of the largest group) and the
+ * shared-memory limit of kb200_execute_knn_* (KB200_EBADARG / KB200_EUNSUPPORTED); a singular local system is
+ * KB200_ESINGULAR. */
+int kb200_lgo(kb200_handle h, const int32_t* group, int n_groups, double* z, double* sigmasq);
+int kb200_knn_lgo(kb200_handle h, int k, const int32_t* group, int n_groups, double* z, double* sigmasq);
+
 /* Debug/verification taps (used by tests only): copy device intermediates to host.
  *  what = 1: Cholesky factor L of the shifted covariance matrix (n_pad x n_pad, row-major, lower triangle valid)
  *  what = 2: W = inv(L) (same layout)
  *  what = 3: dual block: Uz (n_pad x (K+1+V), column-major: C^-1 F for the K+1 drift and unbiasedness columns, then
  *            zeta_v = C^-1 Z_v for the V value fields, V = 1 without kb200_set_values), then Sinv ((K+1)^2), then
  *            phi_1 .. phi_V (K+1 each, phi_v = F^T zeta_v), then c0
+ *  what = 4: G = C^-1 = W^T W as the last kb200_lgo call formed it (same layout as what = 1, lower triangle valid)
  * `cap` is the capacity of `out` in doubles; returns the number of doubles written or a negative code. */
 int64_t kb200_debug_fetch(kb200_handle h, int what, double* out, int64_t cap);
 

@@ -8,6 +8,7 @@ and 'functional' drift terms of the universal classes and output shaping (ok.py:
 dimensions and the classes is data: the class attributes of Krige2D / Krige3D and of the four classes.
 """
 import hashlib
+import re
 import warnings
 from collections import namedtuple
 
@@ -805,6 +806,48 @@ class KrigeBase:
         def run(chunk):
             h = self._ensure_problem("float64", knn, fields=chunk)
             return h.knn_loo(int(n_closest_points), n) if knn else h.loo(n)
+        z, ss = self._per_chunk(fields, run)
+        return (z[0] if one else z), ss
+
+    # ---- leave_group_out(): cross-validation by groups of stations (k-fold, spatial blocks) -------------------
+    def _leave_group_out(self, groups, n_closest_points, values, backend):
+        """(zvalues, sigmasq) of kriging every station from the stations outside its group with this object's fixed
+        variogram (DESIGN.md §5f). groups: N labels of any type np.unique sorts; the errors name the user's label.
+        The problem (and on the global path its factorisation) is shared with execute() and leave_one_out()."""
+        self._check_backend(backend, self._KIND)
+        n = int(np.size(self._data_arrays()[3]))
+        g = np.asarray(groups)
+        if g.ndim != 1 or g.shape[0] != n:
+            raise ValueError("groups must have shape (N,) = (%d,), one label per data point, got shape %s"
+                             % (n, g.shape))
+        labels, dense, sizes = np.unique(g, return_inverse=True, return_counts=True)
+        if labels.size < 2:
+            raise ValueError("leave-group-out needs at least two distinct groups, got %d" % labels.size)
+        dense = np.ascontiguousarray(dense.reshape(-1), dtype=np.int32)
+        knn = n_closest_points is not None
+        if knn:
+            big = int(np.argmax(sizes))
+            if not 2 <= n_closest_points <= n - int(sizes[big]):
+                raise ValueError("leave-group-out: n_closest_points must be in [2, N - %d] = [2, %d] (group %r has %d "
+                                 "stations), got %r" % (sizes[big], n - sizes[big], labels[big].item(), sizes[big],
+                                                        n_closest_points))
+        elif bool(getattr(self, "pseudo_inv", False)):
+            raise NotImplementedError("leave_group_out() has no pseudo_inv=True form on the global path: the "
+                                      "leave-group-out identities need the inverse of the kriging matrix")
+        fields, one = self._check_values(values, "float64", n_closest_points, None)
+
+        def run(chunk):
+            h = self._ensure_problem("float64", knn, fields=chunk)
+            try:
+                if knn:
+                    return h.knn_lgo(int(n_closest_points), dense, labels.size, n)
+                return h.lgo(dense, labels.size, n)
+            except np.linalg.LinAlgError as e:
+                msg = re.sub(r"group (\d+)", lambda m: "group %r" % (labels[int(m.group(1))].item(),), str(e))
+                if labels.size == n:            # every group one station: the leave-one-out message names the station
+                    msg = re.sub(r"station (\d+)", lambda m: "station %s (group %r)" % (
+                        m.group(1), labels[dense[int(m.group(1))]].item()), msg)
+                raise np.linalg.LinAlgError(msg) from None
         z, ss = self._per_chunk(fields, run)
         return (z[0] if one else z), ss
 

@@ -38,7 +38,8 @@ EXPORTS = [
     "kb200_set_problem_knn",
     "kb200_blob_bytes", "kb200_blob_ptr", "kb200_describe_problem", "kb200_blob_commit",
     "kb200_set_coordinates", "kb200_set_stream", "kb200_last_timings", "kb200_reset_counters", "kb200_debug_fetch",
-    "kb200_experimental_variogram", "kb200_statistics", "kb200_loo", "kb200_knn_loo", "kb200_set_pseudo_inverse",
+    "kb200_experimental_variogram", "kb200_statistics", "kb200_loo", "kb200_knn_loo", "kb200_lgo", "kb200_knn_lgo",
+    "kb200_set_pseudo_inverse",
     "kb200_set_variogram_table", "kb200_set_device_drift", "kb200_set_values",
     "kb200_group_create", "kb200_group_destroy", "kb200_group_last_error", "kb200_group_size", "kb200_group_member",
     "kb200_group_set_problem", "kb200_group_set_problem_knn", "kb200_group_execute_points",
@@ -103,6 +104,8 @@ def load_library():
     lib.kb200_statistics.argtypes = [h, dp, dp]
     lib.kb200_loo.argtypes = [h, dp, dp]
     lib.kb200_knn_loo.argtypes = [h, i32, dp, dp]
+    lib.kb200_lgo.argtypes = [h, dp, i32, dp, dp]
+    lib.kb200_knn_lgo.argtypes = [h, i32, dp, i32, dp, dp]
     lib.kb200_set_pseudo_inverse.argtypes = [h, i32]
     lib.kb200_set_variogram_table.argtypes = [h, i64, ctypes.c_double, dp]
     lib.kb200_set_device_drift.argtypes = [h, i32, dp, i64, i64, dp, dp, dp]
@@ -431,6 +434,21 @@ class Handle(_Binding):
         """Moving-window leave-one-out of every station with k neighbours from the other n - 1 (kb200_knn_loo)."""
         z, ss = self._outputs(n)
         self._check(self.lib.kb200_knn_loo(self._h, int(k), _ptr(z), _ptr(ss)), knn=True)
+        return z, ss
+
+    def lgo(self, group, n_groups, n):
+        """Leave-group-out of every station of the problem kb200_set_problem factored on this handle (kb200_lgo):
+        group = n dense group indices in [0, n_groups); (z, sigmasq) as loo()."""
+        g = np.ascontiguousarray(group, dtype=np.int32)
+        z, ss = self._outputs(n)
+        self._check(self.lib.kb200_lgo(self._h, _ptr(g), int(n_groups), _ptr(z), _ptr(ss)))
+        return z, ss
+
+    def knn_lgo(self, k, group, n_groups, n):
+        """Moving-window leave-group-out: k neighbours from the stations outside each station's group (kb200_knn_lgo)."""
+        g = np.ascontiguousarray(group, dtype=np.int32)
+        z, ss = self._outputs(n)
+        self._check(self.lib.kb200_knn_lgo(self._h, int(k), _ptr(g), int(n_groups), _ptr(z), _ptr(ss)), knn=True)
         return z, ss
 
     def debug_fetch(self, what, count):

@@ -114,6 +114,8 @@ struct kb200_ctx {
     DevBuf kSorted, kCells, kFields;
     DevBuf wVario;            // constructor-side helpers (experimental variogram, statistics)
     DevBuf wLoo;              // leave-one-out workspace
+    DevBuf wLgo, wLgoM;       // leave-group-out: blocks and lists | padded matrices of a large group
+    const int* lgo_sg = nullptr; const int* lgo_qg = nullptr;   // moving-window leave-group-out: groups (sorted | original)
     DevBuf wTab;              // KB200_VG_TABLE: (value, slope) pairs on the device
     std::vector<double> htab; // ... and on the host (value, slope interleaved), for the covariance shift
     double tab_dmax = 0.0; int tab_n = 0;
@@ -210,7 +212,7 @@ extern "C" void kb200_destroy(kb200_handle h) {
     cudaStreamSynchronize(h->stream);
     for (DevBuf* b : {&h->blob, &h->wC, &h->wW, &h->wT, &h->wF, &h->wRaw, &h->wFlag,
                       &h->wPts, &h->wOut, &h->wDrift, &h->wScratch, &h->wFstage, &h->kSorted, &h->kCells, &h->kFields, &h->wVario, &h->wTab,
-                      &h->wLoo, &h->wWells, &h->wExt}) b->release();
+                      &h->wLoo, &h->wLgo, &h->wLgoM, &h->wWells, &h->wExt}) b->release();
     for (int i = 0; i < 2; ++i) {
         if (h->pin[i]) cudaFreeHost(h->pin[i]);
         if (h->evk[i]) cudaEventDestroy(h->evk[i]);
@@ -1008,7 +1010,8 @@ static int run_knn(kb200_ctx* h, int k, const Src& s, double* d_z, double* d_ss,
         kp.r0 = (int)std::min(64.0, std::max(1.0, std::ceil(R)));
     }
     kp.ps = s.point_source(); kp.m = s.count; kp.z_out = d_z; kp.ss_out = d_ss; kp.flag = h->wFlag.as<int>(); kp.zstride = h->zstride;
-    CU(h, kbk_knn_solve(kp, chol, st, loo));
+    if (loo == 2) CU(h, kbk_knn_solve_lgo(kp, chol, h->lgo_sg, h->lgo_qg, st));
+    else CU(h, kbk_knn_solve(kp, chol, st, loo));
     h->launches += 1; h->solve_launches += 1;
     return KB200_OK;
 }
@@ -1398,6 +1401,7 @@ extern "C" int64_t kb200_debug_fetch(kb200_handle h, int what, double* out, int6
     const void* src = nullptr; size_t cnt = 0;
     if (what == 1) { src = h->wC.p; cnt = mat; }
     else if (what == 2) { src = h->wW.p; cnt = mat; }
+    else if (what == 4) { src = h->wT.p; cnt = mat; }     // G = W^T W after a kb200_lgo call (gform 0)
     else if (what == 3) {
         size_t nU = (size_t)h->na * h->n_pad;
         size_t nc = (size_t)h->K1 * h->na;            // Sinv ((K+1)^2) | phi_v ((K+1) per field)
@@ -1507,4 +1511,237 @@ extern "C" int kb200_knn_loo(kb200_handle h, int k, double* z_out, double* ss_ou
     // the stations' raw coordinates are the query points
     const Src s{false, 0, 0, 0, raw_col(h, RAW_X), raw_col(h, RAW_Y), raw_col(h, RAW_Z), 0, h->n, nullptr, 0, 0};
     return knn_to_host(h, k, s, z_out, ss_out, 1);
+}
+
+// ---- leave-group-out cross-validation (DESIGN.md §5f) ---------------------------------------------------------------
+// group[i] in [0, n_groups), n_groups >= 2, no empty group; sizes[g] = stations of group g
+static int check_groups(kb200_ctx* h, const int32_t* group, int n_groups, std::vector<int>& sizes) {
+    if (!group) return fail(h, KB200_EBADARG, "null pointer");
+    if (n_groups < 2 || n_groups > h->n) return fail(h, KB200_EBADARG, "leave-group-out: n_groups must be in [2, n]");
+    sizes.assign(n_groups, 0);
+    for (int i = 0; i < h->n; ++i) {
+        if (group[i] < 0 || group[i] >= n_groups)
+            return fail(h, KB200_EBADARG, "leave-group-out: group of station " + std::to_string(i) + " outside [0, n_groups)");
+        ++sizes[group[i]];
+    }
+    for (int g = 0; g < n_groups; ++g)
+        if (!sizes[g]) return fail(h, KB200_EBADARG, "leave-group-out: group " + std::to_string(g) + " is empty");
+    return KB200_OK;
+}
+
+extern "C" int kb200_lgo(kb200_handle h, const int32_t* group, int n_groups, double* z_out, double* ss_out) {
+    if (!h || !z_out || !ss_out) return KB200_EBADARG;
+    if (!h->ready) return fail(h, KB200_ESTATE, "no factored problem: call kb200_set_problem first");
+    if (h->gform == 2) return fail(h, KB200_EUNSUPPORTED, "leave-group-out needs the inverse of the kriging matrix; "
+                                   "the pseudo-inverse (pseudo_inv=True) does not give it");
+    if (!h->local_factor) return fail(h, KB200_ESTATE, "the factorisation is not on this handle "
+                                      "(problem received through kb200_blob_commit)");
+    std::vector<int> sizes;
+    int rc = check_groups(h, group, n_groups, sizes); if (rc) return rc;
+    if (n_groups == h->n) return kb200_loo(h, z_out, ss_out);      // every group a singleton: leave-one-out
+    cudaSetDevice(h->device);
+    cudaStream_t st = h->stream;
+    const int nn = h->n, np = h->n_pad, ld = h->ld, nv = h->nf ? h->nf : 1;
+    const BlobView b = blob_view(h);
+    int launches = 0;
+
+    // host lists: stations group by group (ascending inside a group), positions, block offsets, small / large groups
+    std::vector<int> goff(n_groups + 1, 0), mem(nn), pos(nn), small, large;
+    std::vector<long long> boff(n_groups);
+    for (int g = 0; g < n_groups; ++g) goff[g + 1] = goff[g] + sizes[g];
+    {
+        std::vector<int> cur(goff.begin(), goff.end() - 1);
+        for (int i = 0; i < nn; ++i) { pos[i] = cur[group[i]] - goff[group[i]]; mem[cur[group[i]]++] = i; }
+    }
+    long long nblk = 0; int max_small = 0, max_m = 0;
+    for (int g = 0; g < n_groups; ++g) {
+        boff[g] = nblk; nblk += (long long)sizes[g] * sizes[g];
+        max_m = std::max(max_m, sizes[g]);
+        if (sizes[g] <= LGO_SMALL) { small.push_back(g); max_small = std::max(max_small, sizes[g]); }
+        else large.push_back(g);
+    }
+
+    // exact_values: near pairs of stations in different groups (the pairs inside a group are held out together)
+    std::vector<int> dst, doff(1, 0), dj; std::vector<double> dd; std::vector<long long> soff(1, 0);
+    if (h->vg.exact) {
+        CU(h, h->wLoo.reserve((size_t)(2 * nn + 1) * sizeof(int)));
+        int* cnt = h->wLoo.as<int>();
+        int* off = cnt + nn;
+        CU(h, kbk_loo_pairs(h->dim, nn, b.ax, b.ay, b.az, h->vg.eps, cnt, nullptr, nullptr, nullptr, st)); ++launches;
+        std::vector<int> hcnt(nn), hoff(nn + 1, 0);
+        CU(h, cudaMemcpyAsync(hcnt.data(), cnt, (size_t)nn * sizeof(int), cudaMemcpyDeviceToHost, st));
+        CU(h, cudaStreamSynchronize(st));
+        for (int i = 0; i < nn; ++i) hoff[i + 1] = hoff[i] + hcnt[i];
+        if (hoff[nn] > 0) {
+            const size_t tot = (size_t)hoff[nn];
+            CU(h, h->wVario.reserve(tot * (sizeof(double) + sizeof(int))));
+            double* pd = h->wVario.as<double>();
+            int* pj = reinterpret_cast<int*>(pd + tot);
+            CU(h, cudaMemcpyAsync(off, hoff.data(), (size_t)(nn + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
+            CU(h, kbk_loo_pairs(h->dim, nn, b.ax, b.ay, b.az, h->vg.eps, cnt, off, pj, pd, st)); ++launches;
+            std::vector<int> hpj(tot); std::vector<double> hpd(tot);
+            CU(h, cudaMemcpyAsync(hpj.data(), pj, tot * sizeof(int), cudaMemcpyDeviceToHost, st));
+            CU(h, cudaMemcpyAsync(hpd.data(), pd, tot * sizeof(double), cudaMemcpyDeviceToHost, st));
+            CU(h, cudaStreamSynchronize(st));
+            for (int i = 0; i < nn; ++i) {
+                int c = 0;
+                for (int t = hoff[i]; t < hoff[i + 1]; ++t)
+                    if (group[hpj[t]] != group[i]) { dj.push_back(hpj[t]); dd.push_back(hpd[t]); ++c; }
+                if (!c) continue;
+                if (c > LOO_MAXDUP)
+                    return fail(h, KB200_EUNSUPPORTED, "leave-group-out: station " + std::to_string(i) + " has " +
+                                std::to_string(c) + " stations of other groups within eps (at most " +
+                                std::to_string(LOO_MAXDUP) + ")");
+                dst.push_back(i); doff.push_back((int)dj.size());
+                soff.push_back(soff.back() + 2LL * c * sizes[group[i]]);
+            }
+        }
+    }
+    const int nst = (int)dst.size();
+
+    // workspace (doubles): blk | scale [n] | alpha [nv][n] | e [nv][n] | z [nv][n] | ss [n] | pii [n] |
+    // dd | dup scratch; then long long: boff | soff; then int: grp | mem | goff | pos | small | dst | doff | dj | bad
+    const size_t ndbl = (size_t)nblk + (size_t)nn * (3 + 3 * (size_t)nv) + dd.size() + (size_t)soff.back();
+    const size_t nll = boff.size() + soff.size();
+    const size_t nint = 3 * (size_t)nn + goff.size() + small.size() + dst.size() + doff.size() + dj.size() + 2;
+    CU(h, h->wLgo.reserve(ndbl * 8 + nll * 8 + nint * 4 + 256));
+    double* blk = h->wLgo.as<double>();
+    double* scale = blk + nblk;
+    double* alpha = scale + nn;
+    double* de = alpha + (size_t)nv * nn;
+    double* dz = de + (size_t)nv * nn;
+    double* dss = dz + (size_t)nv * nn;
+    double* lpii = dss + nn;
+    double* ddd = lpii + nn;
+    double* dscr = ddd + dd.size();
+    long long* dboff = reinterpret_cast<long long*>(dscr + soff.back());
+    long long* dsoff = dboff + boff.size();
+    int* dgrp = reinterpret_cast<int*>(dsoff + soff.size());
+    int* dmem = dgrp + nn; int* dgoff = dmem + nn; int* dpos = dgoff + goff.size(); int* dsmall = dpos + nn;
+    int* ddst = dsmall + small.size(); int* ddoff = ddst + dst.size(); int* ddj = ddoff + doff.size();
+    int* bad = ddj + dj.size(); int* lbad = bad + 1;
+    auto up = [&](void* d, const void* s, size_t bytes) {
+        return bytes ? cudaMemcpyAsync(d, s, bytes, cudaMemcpyHostToDevice, st) : cudaSuccess;
+    };
+    CU(h, up(dgrp, group, (size_t)nn * 4)); CU(h, up(dmem, mem.data(), (size_t)nn * 4));
+    CU(h, up(dgoff, goff.data(), goff.size() * 4)); CU(h, up(dpos, pos.data(), (size_t)nn * 4));
+    CU(h, up(dsmall, small.data(), small.size() * 4)); CU(h, up(dboff, boff.data(), boff.size() * 8));
+    CU(h, up(ddst, dst.data(), dst.size() * 4)); CU(h, up(ddoff, doff.data(), doff.size() * 4));
+    CU(h, up(ddj, dj.data(), dj.size() * 4)); CU(h, up(ddd, dd.data(), dd.size() * 8));
+    CU(h, up(dsoff, soff.data(), soff.size() * 8));
+    const int big = INT_MAX;
+    CU(h, up(bad, &big, 4));
+
+    // G = C^-1: W^T W into wT (free after kb200_set_problem), or the Gauss-Jordan inverse already in wC
+    CU(h, cudaEventRecord(h->ev[EV_RUN], st));
+    const double* G = h->wC.as<double>();
+    if (h->gform == 0) {
+        CU(h, kbk_gram_lower(h->wW.as<double>(), ld, np, h->wT.as<double>(), ld, st)); ++launches;
+        G = h->wT.as<double>();
+    }
+    CU(h, cudaEventRecord(h->ev[EV_INVERT], st));
+    // alpha_v = P Z_v: the leave-one-out finalize on G (its other outputs are overwritten below)
+    LooParams lp{};
+    lp.n = nn; lp.n_pad = np; lp.ld = ld; lp.K1 = h->K1; lp.nv = nv; lp.gform = 1; lp.nchunks = 0;
+    lp.tol = KB_LOO_TOL; lp.vg = h->vg; lp.G = G; lp.Uz = aux_block(h, AUX_U); lp.consts = b.consts;
+    lp.Z = kriged_values(h); lp.pii = lpii; lp.alpha = alpha; lp.z_out = dz; lp.ss_out = dss; lp.bad = lbad;
+    LgoParams p{};
+    p.n = nn; p.n_pad = np; p.ld = ld; p.K1 = h->K1; p.nv = nv; p.tol = KB_LOO_TOL; p.vg = h->vg;
+    p.G = G; p.Uz = lp.Uz; p.consts = b.consts; p.Z = lp.Z; p.alpha = alpha;
+    p.grp = dgrp; p.mem = dmem; p.goff = dgoff; p.pos = dpos; p.boff = dboff; p.blk = blk; p.scale = scale; p.e = de;
+    p.z_out = dz; p.ss_out = dss; p.bad = bad;
+    CU(h, kbk_loo_finalize(lp, st)); ++launches;
+    CU(h, kbk_lgo_gather(p, n_groups, max_m, st)); ++launches;
+    CU(h, kbk_lgo_small(p, (int)small.size(), dsmall, max_small, st)); launches += small.empty() ? 0 : 1;
+
+    // large groups, one after another in one padded workspace: Cholesky -> triangular inverse -> W^T W, or Gauss-Jordan.
+    // The padding's diagonal is the group's largest scale, so that it never looks like a pivot at rounding level.
+    int large_bad = big;
+    if (!large.empty()) {
+        std::vector<double> hscale(nn);
+        CU(h, cudaMemcpyAsync(hscale.data(), scale, (size_t)nn * 8, cudaMemcpyDeviceToHost, st));
+        CU(h, cudaStreamSynchronize(st));
+        const int mp = (int)align_up((size_t)max_m, 64);
+        const size_t mat = (size_t)mp * mp;
+        CU(h, h->wLgoM.reserve(3 * mat * sizeof(double) + 256));
+        double* A = h->wLgoM.as<double>();
+        double* Wm = A + mat;
+        double* T1 = Wm + mat;
+        int* flag = reinterpret_cast<int*>(T1 + mat);
+        if (h->gform == 1) CU(h, h->wVario.reserve(kbk_general_inverse_workspace_bytes(mp)));
+        if (!h->hi_stream) {
+            int lo = 0, hi = 0;
+            CU(h, cudaDeviceGetStreamPriorityRange(&lo, &hi));
+            CU(h, cudaStreamCreateWithPriority(&h->hi_stream, cudaStreamNonBlocking, hi));
+        }
+        const size_t need = 2 * (size_t)((mp / 64 + 3) / 4) + 1;
+        while (h->fev.size() < need) {
+            cudaEvent_t e;
+            CU(h, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+            h->fev.push_back(e);
+        }
+        for (int g : large) {
+            const int m = sizes[g], gp = (int)align_up((size_t)m, 64);
+            double smax = 0.0;
+            for (int a = goff[g]; a < goff[g + 1]; ++a) smax = std::max(smax, hscale[a]);
+            if (!(smax > 0.0)) smax = 1.0;
+            int hflag = 0;
+            CU(h, cudaMemsetAsync(flag, 0, sizeof(int), st));
+            CU(h, kbk_lgo_pad(blk + boff[g], m, A, gp, smax, st)); ++launches;
+            if (h->gform == 0) {
+                CU(h, kbk_cholesky(A, Wm, T1, gp, gp, flag, KB_LOO_TOL * smax, st, h->hi_stream, h->fev.data(),
+                                   (int)h->fev.size(), &launches));
+                CU(h, kbk_trtri(A, Wm, T1, gp, gp, st, &launches));
+                CU(h, kbk_gram_lower(Wm, gp, gp, A, gp, st)); ++launches;
+            } else {
+                CU(h, kbk_general_inverse(A, gp, gp, h->wVario.p, flag, KB_LOO_TOL * smax, st, &launches));
+            }
+            CU(h, kbk_lgo_unpad(A, gp, blk + boff[g], m, st)); ++launches;
+            CU(h, cudaMemcpyAsync(&hflag, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
+            CU(h, cudaStreamSynchronize(st));
+            if (hflag != 0) { large_bad = g; break; }           // ascending order: the lowest large group that fails
+        }
+    }
+    CU(h, cudaEventRecord(h->ev[EV_DUAL], st));
+    CU(h, kbk_lgo_finalize(p, st)); ++launches;
+    if (nst) { CU(h, kbk_lgo_dup(p, nst, ddst, ddoff, ddj, ddd, dsoff, dscr, st)); ++launches; }
+    CU(h, cudaEventRecord(h->ev[EV_RUN_END], st));
+    int hbad = big;
+    CU(h, cudaMemcpyAsync(&hbad, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaMemcpyAsync(z_out, dz, (size_t)nv * nn * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaMemcpyAsync(ss_out, dss, (size_t)nn * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    hbad = std::min(hbad, large_bad);
+    h->tm[TM_SOLVE] += ev_ms(h->ev[EV_RUN], h->ev[EV_RUN_END]);
+    h->tm[TM_TRTRI] += ev_ms(h->ev[EV_RUN], h->ev[EV_INVERT]);       // the Gram product W^T W
+    h->tm[TM_FINALIZE] += ev_ms(h->ev[EV_INVERT], h->ev[EV_DUAL]);   // alpha, the blocks and their inverses
+    h->launches += launches; h->solve_launches += launches;
+    if (hbad != big)
+        return fail(h, KB200_ESINGULAR, "leave-group-out: without group " + std::to_string(hbad) + " (lowest station " +
+                    std::to_string(mem[goff[hbad]]) + ") the drift terms are not determined (singular drift block)");
+    return KB200_OK;
+}
+
+extern "C" int kb200_knn_lgo(kb200_handle h, int k, const int32_t* group, int n_groups, double* z_out, double* ss_out) {
+    int rc = check_knn(h, k); if (rc) return rc;
+    if (!z_out || !ss_out) return fail(h, KB200_EBADARG, "null pointer");
+    std::vector<int> sizes;
+    rc = check_groups(h, group, n_groups, sizes); if (rc) return rc;
+    const int gmax = (int)(std::max_element(sizes.begin(), sizes.end()) - sizes.begin());
+    if (k > h->n - sizes[gmax])
+        return fail(h, KB200_EBADARG, "leave-group-out: n_closest_points must be at most n - " + std::to_string(sizes[gmax]) +
+                    " (the size of group " + std::to_string(gmax) + ")");
+    const int nn = h->n;
+    CU(h, h->wLgo.reserve((size_t)2 * nn * sizeof(int)));
+    int* qg = h->wLgo.as<int>();
+    int* sg = qg + nn;
+    const int* sorig = reinterpret_cast<const int*>(h->kSorted.as<double>() + 4 * (size_t)nn);
+    CU(h, cudaMemcpyAsync(qg, group, (size_t)nn * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    CU(h, kbk_knn_sort_groups(nn, sorig, qg, sg, h->stream));
+    h->launches += 1;
+    h->lgo_sg = sg; h->lgo_qg = qg;
+    const Src s{false, 0, 0, 0, raw_col(h, RAW_X), raw_col(h, RAW_Y), raw_col(h, RAW_Z), 0, h->n, nullptr, 0, 0};
+    rc = knn_to_host(h, k, s, z_out, ss_out, 2);
+    h->lgo_sg = nullptr; h->lgo_qg = nullptr;
+    return rc;
 }

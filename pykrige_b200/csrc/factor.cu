@@ -70,9 +70,9 @@ __global__ void __launch_bounds__(256) assemble_kernel(VgParams vg, int n, int n
 }
 
 // ---------------------------------------------------------------------------
-// 64x64 DMMA GEMM tile core used by the Cholesky trailing update and the
-// triangular inverse: acc(64x64) += A(64 x [k0,k1)) * B([k0,k1) x 64).
-//   A row-major (lda).  B: NN -> B[k*ldb + j];  NT -> Bt[j*ldb + k].
+// 64x64 DMMA GEMM tile core used by the Cholesky trailing update, the
+// triangular inverse and the Gram product W^T W: acc(64x64) += A(64 x [k0,k1)) * B([k0,k1) x 64).
+//   A row-major (lda);  TA -> At[k*lda + i].  B: NN -> B[k*ldb + j];  NT -> Bt[j*ldb + k].
 // 128 threads = 4 warps (2x2), each warp a 32x32 sub-tile = 4x4 m8n8k4 tiles.
 // smem rows are padded (+4 doubles) so the 8x4 / 4x8 fragment reads are conflict-free.
 #define GT_LDS_A 20
@@ -82,7 +82,7 @@ struct GemmSmem {
     double b[64 * GT_LDS_A > 16 * GT_LDS_BN ? 64 * GT_LDS_A : 16 * GT_LDS_BN];
 };
 
-template <bool NT>
+template <bool NT, bool TA = false>
 __device__ __forceinline__ void gemm_tile_64(double (&acc)[4][4][2], GemmSmem& sm,
                                              const double* __restrict__ A, int lda,
                                              const double* __restrict__ B, int ldb,
@@ -95,9 +95,15 @@ __device__ __forceinline__ void gemm_tile_64(double (&acc)[4][4][2], GemmSmem& s
     const int bk = tid >> 3, bj = (tid & 7) * 8;
     double ra[8], rb[8];
     auto gload = [&](int k) {
-        const double* pa = A + (size_t)ar * lda + k + ah;
+        if (TA) {                                      // At tile 16x64: the NN-B mapping
+            const double* pa = A + (size_t)(k + bk) * lda + bj;
 #pragma unroll
-        for (int q = 0; q < 8; ++q) ra[q] = pa[q];
+            for (int q = 0; q < 8; ++q) ra[q] = pa[q];
+        } else {
+            const double* pa = A + (size_t)ar * lda + k + ah;
+#pragma unroll
+            for (int q = 0; q < 8; ++q) ra[q] = pa[q];
+        }
         if (NT) {
             const double* pb = B + (size_t)ar * ldb + k + ah;
 #pragma unroll
@@ -112,8 +118,13 @@ __device__ __forceinline__ void gemm_tile_64(double (&acc)[4][4][2], GemmSmem& s
     gload(k0);
     for (int k = k0; k < k1; k += 16) {
         __syncthreads();   // previous tile fully consumed
+        if (TA) {
 #pragma unroll
-        for (int q = 0; q < 8; ++q) sm.a[ar * GT_LDS_A + ah + q] = ra[q];
+            for (int q = 0; q < 8; ++q) sm.a[(bj + q) * GT_LDS_A + bk] = ra[q];
+        } else {
+#pragma unroll
+            for (int q = 0; q < 8; ++q) sm.a[ar * GT_LDS_A + ah + q] = ra[q];
+        }
         if (NT) {
 #pragma unroll
             for (int q = 0; q < 8; ++q) sm.b[ar * GT_LDS_A + ah + q] = rb[q];
@@ -441,6 +452,20 @@ __global__ void __launch_bounds__(128) trtri_step2_kernel(double* __restrict__ W
 }
 
 // ---------------------------------------------------------------------------
+// Gram product of the triangular inverse (LAPACK lauum): G = W^T W = C^-1 for W = L^-1, lower tiles only,
+//     G_IJ = sum_{K >= I} W_KI^T W_KJ    (I >= J; W_KI = 0 for K < I, and the diagonal tiles of W are lower triangular)
+// One CTA per lower tile, k over the rows [64 I, n_pad) of W in a fixed order (leave-group-out, DESIGN.md §5f).
+__global__ void __launch_bounds__(128) gram_lower_kernel(const double* __restrict__ W, int ld, int n_pad,
+                                                         double* __restrict__ G, int ldg) {
+    __shared__ GemmSmem sm;
+    const int tj = blockIdx.x, ti = blockIdx.y;
+    if (tj > ti) return;
+    double acc[4][4][2] = {};
+    gemm_tile_64<false, true>(acc, sm, W + ti * 64, ld, W + tj * 64, ld, ti * 64, n_pad);
+    gemm_tile_store(acc, G + (size_t)ti * 64 * ldg + tj * 64, ldg, 1.0, 0.0);
+}
+
+// ---------------------------------------------------------------------------
 // K2c  dual vectors.  Fz (n x na, column-major, column stride n_pad) holds the drift
 // columns, the ones column and the data values.  Hz = W Fz ; Uz = W^T Hz = C^-1 Fz.
 // Regional-linear columns are built on device from the adjusted coordinates
@@ -694,6 +719,12 @@ cudaError_t kbk_trtri(const double* L, double* W, double* T1, int ld, int n_pad,
         trtri_step2_kernel<<<grid, 128, 0, st>>>(W, T1, ld, n_pad, m);
         *launches += 2;
     }
+    return cudaGetLastError();
+}
+
+cudaError_t kbk_gram_lower(const double* W, int ld, int n_pad, double* G, int ldg, cudaStream_t st) {
+    const int nb = n_pad / 64;
+    gram_lower_kernel<<<dim3(nb, nb), 128, 0, st>>>(W, ld, n_pad, G, ldg);
     return cudaGetLastError();
 }
 

@@ -287,6 +287,11 @@ cudaError_t kbk_knn_build(int dim, int n, const double* ax, const double* ay, co
 // loo = 1: leave-one-out of every station, query p = station ps.first + p (ps = the raw station coordinates), and the
 // candidate with that original index is never counted
 cudaError_t kbk_knn_solve(const KnnParams& p, int chol, cudaStream_t st, int loo = 0);
+// leave-group-out: as loo = 1, but every candidate whose group (sgroup, cell-sorted) equals the query station's group
+// (qgroup, original order) is never counted
+cudaError_t kbk_knn_solve_lgo(const KnnParams& p, int chol, const int* sgroup, const int* qgroup, cudaStream_t st);
+// dst[s] = src[sorig[s]]: group labels in the cell-sorted order of the moving window
+cudaError_t kbk_knn_sort_groups(int n, const int* sorig, const int* src, int* dst, cudaStream_t st);
 size_t      kbk_knn_smem_per_warp(int k, int chol, int hasz, int nv);
 // dst[v * n + s] = src[v * n + sorig[s]] for v < nv: value fields in the cell-sorted order of the moving window
 cudaError_t kbk_knn_sort_fields(int n, int nv, const int* sorig, const double* src, double* dst, cudaStream_t st);
@@ -329,6 +334,40 @@ cudaError_t kbk_loo_pairs(int dim, int n, const double* ax, const double* ay, co
                           const int* off, int* pj, double* pd, cudaStream_t st);
 cudaError_t kbk_loo_dup(const LooParams& p, int nst, const int* st_list, const int* off, const int* pj, const double* pd,
                         cudaStream_t st);
+
+// loo.cu: leave-group-out cross-validation (DESIGN.md §5f)
+#define LGO_SMALL 128       // largest group whose block is inverted in shared memory (one CTA); larger: blocked kernels
+struct LgoParams {
+    int n, n_pad, ld, K1, nv;
+    double tol;                // a pivot at or below tol * scale of its station: drift not determined without the group
+    VgParams vg;
+    const double* G;           // G = C^-1, lower triangle (row-major, ld)
+    const double* Uz;          // as LooParams
+    const double* consts;
+    const double* Z;
+    const double* alpha;       // [nv][n] alpha_v = P Z_v (loo_finalize_kernel)
+    const int* grp;            // [n] dense group index of each station
+    const int* mem;            // [n] the stations group by group, ascending inside a group
+    const int* goff;           // [n_groups + 1] group g is mem[goff[g] .. goff[g + 1])
+    const int* pos;            // [n] position of each station inside its group
+    const long long* boff;     // [n_groups] start of group g's m x m block in blk
+    double* blk;               // P_SS of every group, then its inverse (row-major)
+    double* scale;             // [n] in mem order: max(|G_ii|, |u_i^T S^-1 u_i|)
+    double* e;                 // [nv][n] e_S,v of each station
+    double* z_out; double* ss_out;   // [nv][n], [n]
+    int* bad;                  // lowest group whose block has a pivot at rounding level (INT_MAX: none)
+};
+// G = W^T W, lower tiles only (factor.cu, DMMA)
+cudaError_t kbk_gram_lower(const double* W, int ld, int n_pad, double* G, int ldg, cudaStream_t st);
+cudaError_t kbk_lgo_gather(const LgoParams& p, int n_groups, int max_m, cudaStream_t st);
+size_t      kbk_lgo_small_smem(int m);
+cudaError_t kbk_lgo_small(const LgoParams& p, int count, const int* glist, int max_m, cudaStream_t st);
+cudaError_t kbk_lgo_pad(const double* blk, int m, double* dst, int ld, double d, cudaStream_t st);   // d: padding diagonal
+cudaError_t kbk_lgo_unpad(const double* src, int ld, double* blk, int m, cudaStream_t st);
+cudaError_t kbk_lgo_finalize(const LgoParams& p, cudaStream_t st);
+// one warp per station of st_list; its near stations of other groups at pj/pd + off[w] (off: [nst + 1])
+cudaError_t kbk_lgo_dup(const LgoParams& p, int nst, const int* st_list, const int* off, const int* pj, const double* pd,
+                        const long long* soff, double* scratch, cudaStream_t st);
 
 // pinv.cu: pseudo_inv=True (one-sided Jacobi SVD of the bordered kriging matrix)
 cudaError_t kbk_build_fz(int n, int n_pad, int n_rl, int n_hd, const double* ax, const double* ay, const double* az,

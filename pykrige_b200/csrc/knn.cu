@@ -123,12 +123,15 @@ __device__ __forceinline__ void warp_bitonic(double* d2, int* id, const int* __r
 //               A non-positive pivot (variogram not valid in this dimension) sets *flag = 2 and the host
 //               re-runs the launch with CHOL = false.
 // CHOL = false: LU with partial pivoting on the full k x k block (dgesv semantics, cok.pyx:165-174).
-// LOO = true : leave-one-out of station q = ps.first + p (ps holds the raw station coordinates): the candidate with
+// MODE 1 (LOO): leave-one-out of station q = ps.first + p (ps holds the raw station coordinates): the candidate with
 //              original index q is never counted. It lands at d^2 == 0 exactly (data and query go through the same
 //              adjust sequence), so only there is its index looked up.
-template <int DIM, int MODEL, bool CHOL, bool LOO = false>
-__global__ void __launch_bounds__(320) knn_solve_kernel(const __grid_constant__ KnnParams P, int warps_per_cta,
-                                                         int per_warp_doubles) {
+// MODE 2 (LGO): leave-group-out: the query is station q as in MODE 1, and every candidate of q's group is never counted
+//              (sgroup: groups in the cell-sorted order, qgroup: in the original order).
+template <int DIM, int MODEL, bool CHOL, int MODE>
+__device__ __forceinline__ void knn_solve_body(const KnnParams& P, int warps_per_cta, int per_warp_doubles,
+                                               const int* __restrict__ sgroup, const int* __restrict__ qgroup) {
+    constexpr bool LOO = MODE == 1;
     extern __shared__ __align__(16) double ksm[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     if (warp >= warps_per_cta) return;
@@ -161,6 +164,7 @@ __global__ void __launch_bounds__(320) knn_solve_kernel(const __grid_constant__ 
 
     double qx, qy, qz;
     kb_load_point<DIM>(P.ps, P.an, p, qx, qy, qz);
+    const int qg = MODE == 2 ? qgroup[P.ps.first + p] : 0;
 
     // ---------------- K4: exact k nearest ----------------
     const int cqx = min(P.gx - 1, max(0, (int)floor((qx - P.ox) * P.inv_cell)));
@@ -222,6 +226,7 @@ __global__ void __launch_bounds__(320) knn_solve_kernel(const __grid_constant__ 
                     d2 = dx * dx + dy * dy;
                     if (KB_HASZ(DIM)) { double dz = P.az[i] - qz; d2 += dz * dz; }
                     if (LOO && d2 == 0.0 && P.sorig[i] == P.ps.first + p) ok = false;
+                    if (MODE == 2 && sgroup[i] == qg) ok = false;
                 }
                 unsigned msk = __ballot_sync(0xffffffffu, ok);
                 int pos = cnt + __popc(msk & ((1u << lane) - 1u));
@@ -671,6 +676,19 @@ __global__ void __launch_bounds__(320) knn_solve_kernel(const __grid_constant__ 
     }
 }
 
+template <int DIM, int MODEL, bool CHOL, bool LOO = false>
+__global__ void __launch_bounds__(320) knn_solve_kernel(const __grid_constant__ KnnParams P, int warps_per_cta,
+                                                         int per_warp_doubles) {
+    knn_solve_body<DIM, MODEL, CHOL, LOO ? 1 : 0>(P, warps_per_cta, per_warp_doubles, nullptr, nullptr);
+}
+
+template <int DIM, int MODEL, bool CHOL>
+__global__ void __launch_bounds__(320) knn_lgo_kernel(const __grid_constant__ KnnParams P, int warps_per_cta,
+                                                       int per_warp_doubles, const int* __restrict__ sgroup,
+                                                       const int* __restrict__ qgroup) {
+    knn_solve_body<DIM, MODEL, CHOL, 2>(P, warps_per_cta, per_warp_doubles, sgroup, qgroup);
+}
+
 // ---- host side -------------------------------------------------------------
 size_t kbk_knn_smem_per_warp(int k, int chol, int hasz, int nv) {
     size_t S = (size_t)(k | 1);
@@ -713,6 +731,35 @@ cudaError_t kbk_knn_solve(const KnnParams& p, int chol, cudaStream_t st, int loo
             });
         });
     });
+}
+
+cudaError_t kbk_knn_solve_lgo(const KnnParams& p, int chol, const int* sgroup, const int* qgroup, cudaStream_t st) {
+    return KbDims::dispatch(p.dim, [&](auto D) {
+        return KbModels::dispatch(p.vg.model, [&](auto M) {
+            return KbBools::dispatch(chol && p.k <= 128, [&](auto CHOL) {
+                const size_t per = kbk_knn_smem_per_warp(p.k, CHOL, KB_HASZ(D) ? 1 : 0, p.nv);
+                const int wpc = (int)std::min<size_t>(10, (size_t)(226 * 1024) / per);
+                if (wpc < 1) return cudaErrorInvalidValue;
+                const size_t smem = per * wpc;
+                KB_CUDA_OK(cudaFuncSetAttribute(knn_lgo_kernel<D, M, bool(CHOL)>,
+                                                cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                knn_lgo_kernel<D, M, bool(CHOL)><<<(unsigned)((p.m + wpc - 1) / wpc), wpc * 32, smem, st>>>(
+                    p, wpc, (int)(per / sizeof(double)), sgroup, qgroup);
+                return cudaGetLastError();
+            });
+        });
+    });
+}
+
+__global__ void knn_sort_groups_kernel(int n, const int* __restrict__ sorig, const int* __restrict__ src,
+                                       int* __restrict__ dst) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s < n) dst[s] = src[sorig[s]];
+}
+
+cudaError_t kbk_knn_sort_groups(int n, const int* sorig, const int* src, int* dst, cudaStream_t st) {
+    knn_sort_groups_kernel<<<(n + 255) / 256, 256, 0, st>>>(n, sorig, src, dst);
+    return cudaGetLastError();
 }
 
 cudaError_t kbk_knn_build(int dim, int n, const double* ax, const double* ay, const double* az, const double* values,

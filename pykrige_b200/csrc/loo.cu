@@ -11,6 +11,7 @@
 #include "common.cuh"
 #include "kernels.h"
 #include <climits>
+#include <algorithm>
 
 #define LOO_CB 128          // columns of W per CTA of the column-norm kernel (one per thread: coalesced row loads)
 
@@ -196,5 +197,241 @@ cudaError_t kbk_loo_dup(const LooParams& p, int nst, const int* st_list, const i
                         cudaStream_t st) {
     if (nst == 0) return cudaSuccess;
     loo_dup_kernel<<<(nst + 7) / 8, 256, 0, st>>>(p, nst, st_list, off, pj, pd);
+    return cudaGetLastError();
+}
+
+// ---- leave-group-out (DESIGN.md §5f) --------------------------------------------------------------------------------
+// For a group S (T: the other stations), with P and alpha as above and G = C^-1 held as a lower triangle:
+//     e_S,v = P_SS^-1 alpha_S,v,   zhat_S,v = Z_S,v - e_S,v,   sigma^2_S = diag(P_SS^-1).
+// The blocks P_SS of all groups are gathered into one array (group g: m_g x m_g, row-major, stations ascending), each is
+// replaced by its inverse (lgo_small_kernel in shared memory, or the blocked factor kernels on a padded copy for a
+// large group), then lgo_finalize_kernel forms e, zhat and sigma^2 and lgo_dup_kernel the exact-hit correction.
+
+// P_jl = G_jl - u_j^T S^-1 u_l, evaluated in the order (max(j, l), min(j, l)) so that P is exactly symmetric;
+// *usu_out = u_j^T S^-1 u_l
+__device__ double lgo_p(const LgoParams& P, int j, int l, double* usu_out = nullptr) {
+    const int hi = max(j, l), lo = min(j, l);
+    const double s = P.G[(size_t)hi * P.ld + lo];
+    const int K1 = P.K1;
+    double usu = 0.0;
+    for (int a = 0; a < K1; ++a) {
+        double t = 0.0;
+        for (int b = 0; b < K1; ++b) t += P.consts[a * K1 + b] * P.Uz[(size_t)b * P.n_pad + lo];
+        usu += P.Uz[(size_t)a * P.n_pad + hi] * t;
+    }
+    if (usu_out) *usu_out = usu;
+    return s - usu;
+}
+
+// blk[boff[g] + a m + b] = P_{S_a S_b} for every group g = blockIdx.y (grid-stride over its m^2 entries); the diagonal also
+// gives scale[goff[g] + a] = max(|G_ii|, |u_i^T S^-1 u_i|), the terms whose difference P_ii is
+__global__ void __launch_bounds__(256) lgo_gather_kernel(LgoParams P) {
+    const int g = blockIdx.y, o = P.goff[g], m = P.goff[g + 1] - o;
+    double* blk = P.blk + P.boff[g];
+    for (long long e = (long long)blockIdx.x * 256 + threadIdx.x; e < (long long)m * m; e += (long long)gridDim.x * 256) {
+        const int a = (int)(e / m), b = (int)(e % m);
+        const int i = P.mem[o + a], j = P.mem[o + b];
+        double usu;
+        blk[e] = lgo_p(P, i, j, &usu);
+        if (a == b) P.scale[o + a] = fmax(fabs(P.G[(size_t)i * P.ld + i]), fabs(usu));
+    }
+}
+
+// In-place Gauss-Jordan inverse of one small block (m <= LGO_SMALL) in shared memory, one CTA per group: partial
+// pivoting (largest |value|, ties to the lower row), the column swaps in reverse order at the end. A pivot at or below
+// tol * scale of its station means the drift is not determined without the group: *bad = lowest such group.
+__global__ void __launch_bounds__(256) lgo_small_kernel(LgoParams P, const int* __restrict__ glist) {
+    extern __shared__ __align__(16) double lsm[];
+    __shared__ double wv[8]; __shared__ int wi[8];
+    __shared__ int fail;
+    const int g = glist[blockIdx.x], o = P.goff[g], m = P.goff[g + 1] - o;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    double* A = lsm;                                 // m x m
+    double* col = A + (size_t)m * m;                 // column k before the update
+    int* piv = reinterpret_cast<int*>(col + m);      // row swapped with row k at step k
+    int* rid = piv + m;                              // position in the group of the row's station
+    double* blk = P.blk + P.boff[g];
+    for (int e = tid; e < m * m; e += 256) A[e] = blk[e];
+    for (int t = tid; t < m; t += 256) rid[t] = t;
+    if (tid == 0) fail = 0;
+    __syncthreads();
+    for (int k = 0; k < m; ++k) {
+        double bv = -1.0; int bi = m;
+        for (int r = k + tid; r < m; r += 256) {
+            const double v = fabs(A[r * m + k]);
+            if (v > bv || (v == bv && r < bi)) { bv = v; bi = r; }
+        }
+        for (int s = 16; s > 0; s >>= 1) {
+            const double ov = __shfl_xor_sync(0xffffffffu, bv, s);
+            const int oi = __shfl_xor_sync(0xffffffffu, bi, s);
+            if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+        }
+        if (lane == 0) { wv[warp] = bv; wi[warp] = bi; }
+        __syncthreads();
+        if (tid == 0) {
+            for (int w = 1; w < 8; ++w)
+                if (wv[w] > bv || (wv[w] == bv && wi[w] < bi)) { bv = wv[w]; bi = wi[w]; }
+            piv[k] = bi;
+        }
+        __syncthreads();
+        const int p = piv[k];
+        if (p != k) {
+            for (int c = tid; c < m; c += 256) { const double t = A[k * m + c]; A[k * m + c] = A[p * m + c]; A[p * m + c] = t; }
+            if (tid == 0) { const int t = rid[k]; rid[k] = rid[p]; rid[p] = t; }
+        }
+        __syncthreads();
+        const double pv = A[k * m + k];
+        const double inv = 1.0 / pv;
+        if (tid == 0 && !(fabs(pv) > P.tol * P.scale[o + rid[k]])) fail = 1;
+        for (int r = tid; r < m; r += 256) col[r] = A[r * m + k];
+        __syncthreads();
+        for (int c = tid; c < m; c += 256) A[k * m + c] = (c == k) ? inv : A[k * m + c] * inv;
+        __syncthreads();
+        for (int e = tid; e < m * m; e += 256) {
+            const int r = e / m, c = e - r * m;
+            if (r == k) continue;
+            A[e] = (c == k) ? -col[r] * inv : A[e] - col[r] * A[k * m + c];
+        }
+        __syncthreads();
+    }
+    for (int k = m - 1; k >= 0; --k) {
+        const int p = piv[k];
+        if (p != k)
+            for (int r = tid; r < m; r += 256) { const double t = A[r * m + k]; A[r * m + k] = A[r * m + p]; A[r * m + p] = t; }
+        __syncthreads();
+    }
+    for (int e = tid; e < m * m; e += 256) blk[e] = A[e];
+    if (tid == 0 && fail) atomicMin(P.bad, g);
+}
+
+// padded copy of a large block for the blocked factor kernels: dst (ld x ld) = [[blk, 0], [0, d I]]
+__global__ void lgo_pad_kernel(const double* __restrict__ blk, int m, double* __restrict__ dst, int ld, double d) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x, r = blockIdx.y;
+    if (c >= ld) return;
+    dst[(size_t)r * ld + c] = (r < m && c < m) ? blk[(size_t)r * m + c] : (r == c ? d : 0.0);
+}
+
+// ... and back: blk[r][c] = src[max(r, c)][min(r, c)] (the lower triangle of the inverse)
+__global__ void lgo_unpad_kernel(const double* __restrict__ src, int ld, double* __restrict__ blk, int m) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x, r = blockIdx.y;
+    if (c >= m) return;
+    blk[(size_t)r * m + c] = src[(size_t)max(r, c) * ld + min(r, c)];
+}
+
+// One thread per station i (group g, position a): e_v = row a of P_SS^-1 . alpha_S,v (b ascending), zhat = Z - e,
+// sigma^2 = (P_SS^-1)_aa. Every product and sum of field v is the same whatever nv is and wherever v sits.
+__global__ void lgo_finalize_kernel(LgoParams P) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P.n) return;
+    const int g = P.grp[i], o = P.goff[g], m = P.goff[g + 1] - o, a = P.pos[i];
+    const double* row = P.blk + P.boff[g] + (size_t)a * m;
+    P.ss_out[i] = row[a];
+    for (int v = 0; v < P.nv; ++v) {
+        const double* al = P.alpha + (size_t)v * P.n;
+        double e = 0.0;
+        for (int b = 0; b < m; ++b) e += row[b] * al[P.mem[o + b]];
+        P.e[(size_t)v * P.n + i] = e;
+        P.z_out[(size_t)v * P.n + i] = P.Z[(size_t)v * P.n + i] - e;
+    }
+}
+
+// Exact-hit correction of station i in S (one warp per station with near stations outside its group), D = D(i) at
+// pj/pd + off[w] (ascending j, at most LOO_MAXDUP), Delta_j = gamma(d_ij), Q = P_SS^-1:
+//     zhat_v  += sum_j Delta_j (alpha_jv - P_jS e_S,v)
+//     sigma^2 += 2 sum_j Delta_j (P_jS Q)_a - sum_{j,l} Delta_j Delta_l (P_jl - P_jS Q P_Sl)
+// scratch + soff[w]: P_jS (|D| x m), then P_jS Q (|D| x m). Lanes split b; sums over b close with a fixed xor tree.
+__device__ __forceinline__ double lgo_warp_sum(double s) {
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    return s;
+}
+
+__global__ void __launch_bounds__(256) lgo_dup_kernel(LgoParams P, int nst, const int* __restrict__ st,
+                                                      const int* __restrict__ off, const int* __restrict__ pj,
+                                                      const double* __restrict__ pd, const long long* __restrict__ soff,
+                                                      double* __restrict__ scratch) {
+    const int w = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (w >= nst) return;
+    const int i = st[w], d0 = off[w], cnt = off[w + 1] - d0;
+    const int g = P.grp[i], o = P.goff[g], m = P.goff[g + 1] - o, a = P.pos[i];
+    const double* Q = P.blk + P.boff[g];
+    double* ps = scratch + soff[w];                  // [cnt][m] P_jS
+    double* qs = ps + (size_t)cnt * m;               // [cnt][m] P_jS Q
+    double dl[LOO_MAXDUP];
+    for (int t = 0; t < cnt; ++t) {
+        dl[t] = loo_gamma(P.vg, pd[d0 + t]);
+        for (int b = lane; b < m; b += 32) ps[(size_t)t * m + b] = lgo_p(P, pj[d0 + t], P.mem[o + b]);
+    }
+    __syncwarp();
+    for (int t = 0; t < cnt; ++t)
+        for (int b = lane; b < m; b += 32) {
+            double s = 0.0;
+            for (int c = 0; c < m; ++c) s += ps[(size_t)t * m + c] * Q[(size_t)c * m + b];
+            qs[(size_t)t * m + b] = s;
+        }
+    __syncwarp();
+    double ds = 0.0, quad = 0.0;
+    for (int t = 0; t < cnt; ++t) {
+        ds += dl[t] * qs[(size_t)t * m + a];
+        for (int u = 0; u < cnt; ++u) {
+            double s = 0.0;
+            for (int b = lane; b < m; b += 32) s += qs[(size_t)t * m + b] * ps[(size_t)u * m + b];
+            s = lgo_warp_sum(s);
+            quad += dl[t] * dl[u] * (lgo_p(P, pj[d0 + t], pj[d0 + u]) - s);
+        }
+    }
+    double dz[KB200_MAX_FIELDS];
+    for (int v = 0; v < P.nv; ++v) {
+        const double* e = P.e + (size_t)v * P.n;
+        double acc = 0.0;
+        for (int t = 0; t < cnt; ++t) {
+            double s = 0.0;
+            for (int b = lane; b < m; b += 32) s += ps[(size_t)t * m + b] * e[P.mem[o + b]];
+            s = lgo_warp_sum(s);
+            acc += dl[t] * (P.alpha[(size_t)v * P.n + pj[d0 + t]] - s);
+        }
+        dz[v] = acc;
+    }
+    if (lane == 0) {
+        P.ss_out[i] += 2.0 * ds - quad;
+        for (int v = 0; v < P.nv; ++v) P.z_out[(size_t)v * P.n + i] += dz[v];
+    }
+}
+
+cudaError_t kbk_lgo_gather(const LgoParams& p, int n_groups, int max_m, cudaStream_t st) {
+    const long long e = (long long)max_m * max_m;
+    const int bx = (int)std::min<long long>(64, (e + 255) / 256);
+    lgo_gather_kernel<<<dim3(bx, n_groups), 256, 0, st>>>(p);
+    return cudaGetLastError();
+}
+
+size_t kbk_lgo_small_smem(int m) { return (size_t)m * m * sizeof(double) + (size_t)m * (sizeof(double) + 2 * sizeof(int)); }
+
+cudaError_t kbk_lgo_small(const LgoParams& p, int count, const int* glist, int max_m, cudaStream_t st) {
+    if (count == 0) return cudaSuccess;
+    const size_t smem = kbk_lgo_small_smem(max_m);
+    KB_CUDA_OK(cudaFuncSetAttribute(lgo_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    lgo_small_kernel<<<count, 256, smem, st>>>(p, glist);
+    return cudaGetLastError();
+}
+
+cudaError_t kbk_lgo_pad(const double* blk, int m, double* dst, int ld, double d, cudaStream_t st) {
+    lgo_pad_kernel<<<dim3((ld + 255) / 256, ld), 256, 0, st>>>(blk, m, dst, ld, d);
+    return cudaGetLastError();
+}
+
+cudaError_t kbk_lgo_unpad(const double* src, int ld, double* blk, int m, cudaStream_t st) {
+    lgo_unpad_kernel<<<dim3((m + 255) / 256, m), 256, 0, st>>>(src, ld, blk, m);
+    return cudaGetLastError();
+}
+
+cudaError_t kbk_lgo_finalize(const LgoParams& p, cudaStream_t st) {
+    lgo_finalize_kernel<<<(p.n + 127) / 128, 128, 0, st>>>(p);
+    return cudaGetLastError();
+}
+
+cudaError_t kbk_lgo_dup(const LgoParams& p, int nst, const int* st_list, const int* off, const int* pj, const double* pd,
+                        const long long* soff, double* scratch, cudaStream_t st) {
+    if (nst == 0) return cudaSuccess;
+    lgo_dup_kernel<<<(nst + 7) / 8, 256, 0, st>>>(p, nst, st_list, off, pj, pd, soff, scratch);
     return cudaGetLastError();
 }

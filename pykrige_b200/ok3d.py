@@ -46,3 +46,18 @@ class OrdinaryKriging3D(Krige3D):
         (NotImplementedError) and ignored by the moving window, as in execute().
         """
         return self._leave_one_out(n_closest_points, values, backend)
+
+    def leave_group_out(self, groups, n_closest_points=None, values=None, backend="cuda"):
+        """Leave-group-out cross-validation: every station kriged from the stations outside its group, with this
+        object's fixed variogram, anisotropy, coordinate type and ``exact_values`` (the variogram is not refitted per
+        fold). ``groups`` is one label per station (N labels of any type ``numpy.unique`` sorts: k random folds,
+        spatial blocks, ...); stations of the same group are held out together. Returns ``(zvalues, sigmasq)`` in station order, shaped as
+        leave_one_out(): ``zvalues`` (N,), or (V, N) for a 2-D ``values``; ``sigmasq`` (N,).
+
+        Without ``n_closest_points`` the global path reads the factorisation the last float64 execute() left on the
+        device (or makes one, which a later execute() reuses) and forms C^-1 once: O(N^3 / 3) plus one small solve per
+        group, not one factorisation per group. ``n_closest_points = k`` runs the moving window with k neighbours from
+        the other groups (2 <= k <= N - size of the largest group). ``values`` as in execute(values=...).
+        ``pseudo_inv=True`` is refused on the global path (NotImplementedError) and ignored by the moving window.
+        """
+        return self._leave_group_out(groups, n_closest_points, values, backend)

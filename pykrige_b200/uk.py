@@ -190,3 +190,17 @@ class UniversalKriging(Krige2D):
         drift terms undetermined, and NotImplementedError with ``pseudo_inv=True``.
         """
         return self._leave_one_out(None, values, backend)
+
+    def leave_group_out(self, groups, values=None, backend="cuda"):
+        """Leave-group-out cross-validation: every station kriged from the stations outside its group, with this
+        object's fixed variogram, anisotropy, drift terms and ``exact_values`` (the variogram is not refitted per
+        fold). ``groups`` is one label per station (N labels of any type ``numpy.unique`` sorts: k random folds,
+        spatial blocks, ...); stations of the same group are held out together. Returns ``(zvalues, sigmasq)`` in station order, shaped as
+        leave_one_out(): ``zvalues`` (N,), or (V, N) for a 2-D ``values``; ``sigmasq`` (N,).
+
+        Reads the factorisation the last float64 execute() left on the device (or makes one, which a later execute()
+        reuses) and forms C^-1 once: O(N^3 / 3) plus one small solve per group, not one factorisation per group.
+        ``values`` as in execute(values=...). Raises ``numpy.linalg.LinAlgError`` naming the group when leaving it
+        out leaves the drift terms undetermined, and NotImplementedError with ``pseudo_inv=True``.
+        """
+        return self._leave_group_out(groups, None, values, backend)
