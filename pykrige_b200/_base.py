@@ -784,60 +784,48 @@ class KrigeBase:
         z, ss = self._per_chunk(fields, run)
         return self._scatter(plan, z, ss)
 
-    # ---- leave_one_out(): cross-validation of every station --------------------------------------------------
-    def _leave_one_out(self, n_closest_points, values, backend):
-        """(zvalues, sigmasq) of kriging every station from the other N - 1 with this object's fixed variogram
-        (DESIGN.md §5e): the global path from the factorisation the last float64 execute() left on the handle (or a
-        new one, which a later execute() reuses), the moving window with n_closest_points neighbours. values as in
-        execute(values=...): zvalues is (V, N) for a 2-D values, (N,) otherwise; sigmasq is (N,)."""
-        self._check_backend(backend, self._KIND)
-        n = int(np.size(self._data_arrays()[3]))
-        if n < 2:
-            raise ValueError("leave-one-out needs at least two data points, got %d" % n)
-        knn = n_closest_points is not None
-        if knn and not 2 <= n_closest_points <= n - 1:
-            raise ValueError("leave-one-out: n_closest_points must be in [2, N - 1] = [2, %d], got %r"
-                             % (n - 1, n_closest_points))
-        if not knn and bool(getattr(self, "pseudo_inv", False)):
-            raise NotImplementedError("leave_one_out() has no pseudo_inv=True form on the global path: the "
-                                      "leave-one-out identities need the inverse of the kriging matrix")
-        fields, one = self._check_values(values, "float64", n_closest_points, None)
-
-        def run(chunk):
-            h = self._ensure_problem("float64", knn, fields=chunk)
-            return h.knn_loo(int(n_closest_points), n) if knn else h.loo(n)
-        z, ss = self._per_chunk(fields, run)
-        return (z[0] if one else z), ss
-
-    # ---- leave_group_out(): cross-validation by groups of stations (k-fold, spatial blocks) -------------------
-    def _leave_group_out(self, groups, n_closest_points, values, backend):
+    # ---- leave_one_out() and leave_group_out(): cross-validation of every station ----------------------------------
+    def _cross_validate(self, groups, n_closest_points, values, backend):
         """(zvalues, sigmasq) of kriging every station from the stations outside its group with this object's fixed
-        variogram (DESIGN.md §5f). groups: N labels of any type np.unique sorts; the errors name the user's label.
-        The problem (and on the global path its factorisation) is shared with execute() and leave_one_out()."""
+        variogram: groups=None holds out each station alone (leave-one-out, DESIGN.md §5e), else groups holds N labels of
+        any type np.unique sorts and the errors name the user's label (leave-group-out, §5f). The global path runs from
+        the factorisation the last float64 execute() left on the handle (or a new one, which a later execute() reuses),
+        the moving window with n_closest_points neighbours. values as in execute(values=...): zvalues is (V, N) for a
+        2-D values, (N,) otherwise; sigmasq is (N,)."""
         self._check_backend(backend, self._KIND)
         n = int(np.size(self._data_arrays()[3]))
-        g = np.asarray(groups)
-        if g.ndim != 1 or g.shape[0] != n:
-            raise ValueError("groups must have shape (N,) = (%d,), one label per data point, got shape %s"
-                             % (n, g.shape))
-        labels, dense, sizes = np.unique(g, return_inverse=True, return_counts=True)
-        if labels.size < 2:
-            raise ValueError("leave-group-out needs at least two distinct groups, got %d" % labels.size)
-        dense = np.ascontiguousarray(dense.reshape(-1), dtype=np.int32)
         knn = n_closest_points is not None
-        if knn:
+        if groups is None:
+            what = "leave-one-out"
+            if n < 2:
+                raise ValueError("leave-one-out needs at least two data points, got %d" % n)
+            if knn and not 2 <= n_closest_points <= n - 1:
+                raise ValueError("leave-one-out: n_closest_points must be in [2, N - 1] = [2, %d], got %r"
+                                 % (n - 1, n_closest_points))
+        else:
+            what = "leave-group-out"
+            g = np.asarray(groups)
+            if g.ndim != 1 or g.shape[0] != n:
+                raise ValueError("groups must have shape (N,) = (%d,), one label per data point, got shape %s"
+                                 % (n, g.shape))
+            labels, dense, sizes = np.unique(g, return_inverse=True, return_counts=True)
+            if labels.size < 2:
+                raise ValueError("leave-group-out needs at least two distinct groups, got %d" % labels.size)
+            dense = np.ascontiguousarray(dense.reshape(-1), dtype=np.int32)
             big = int(np.argmax(sizes))
-            if not 2 <= n_closest_points <= n - int(sizes[big]):
+            if knn and not 2 <= n_closest_points <= n - int(sizes[big]):
                 raise ValueError("leave-group-out: n_closest_points must be in [2, N - %d] = [2, %d] (group %r has %d "
                                  "stations), got %r" % (sizes[big], n - sizes[big], labels[big].item(), sizes[big],
                                                         n_closest_points))
-        elif bool(getattr(self, "pseudo_inv", False)):
-            raise NotImplementedError("leave_group_out() has no pseudo_inv=True form on the global path: the "
-                                      "leave-group-out identities need the inverse of the kriging matrix")
+        if not knn and bool(getattr(self, "pseudo_inv", False)):
+            raise NotImplementedError("%s() has no pseudo_inv=True form on the global path: the %s identities need the "
+                                      "inverse of the kriging matrix" % (what.replace("-", "_"), what))
         fields, one = self._check_values(values, "float64", n_closest_points, None)
 
         def run(chunk):
             h = self._ensure_problem("float64", knn, fields=chunk)
+            if groups is None:
+                return h.knn_loo(int(n_closest_points), n) if knn else h.loo(n)
             try:
                 if knn:
                     return h.knn_lgo(int(n_closest_points), dense, labels.size, n)

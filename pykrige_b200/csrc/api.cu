@@ -115,7 +115,7 @@ struct kb200_ctx {
     DevBuf wVario;            // constructor-side helpers (experimental variogram, statistics)
     DevBuf wLoo;              // leave-one-out workspace
     DevBuf wLgo, wLgoM;       // leave-group-out: blocks and lists | padded matrices of a large group
-    const int* lgo_sg = nullptr; const int* lgo_qg = nullptr;   // moving-window leave-group-out: groups (sorted | original)
+    DevBuf wPairs;            // cross-validation under exact_values: the near-pair lists
     DevBuf wTab;              // KB200_VG_TABLE: (value, slope) pairs on the device
     std::vector<double> htab; // ... and on the host (value, slope interleaved), for the covariance shift
     double tab_dmax = 0.0; int tab_n = 0;
@@ -212,7 +212,7 @@ extern "C" void kb200_destroy(kb200_handle h) {
     cudaStreamSynchronize(h->stream);
     for (DevBuf* b : {&h->blob, &h->wC, &h->wW, &h->wT, &h->wF, &h->wRaw, &h->wFlag,
                       &h->wPts, &h->wOut, &h->wDrift, &h->wScratch, &h->wFstage, &h->kSorted, &h->kCells, &h->kFields, &h->wVario, &h->wTab,
-                      &h->wLoo, &h->wLgo, &h->wLgoM, &h->wWells, &h->wExt}) b->release();
+                      &h->wLoo, &h->wLgo, &h->wLgoM, &h->wPairs, &h->wWells, &h->wExt}) b->release();
     for (int i = 0; i < 2; ++i) {
         if (h->pin[i]) cudaFreeHost(h->pin[i]);
         if (h->evk[i]) cudaEventDestroy(h->evk[i]);
@@ -617,6 +617,22 @@ static int factor_cholesky_pack(kb200_ctx* h, const BlobView& b, int* launches) 
     return 0;
 }
 
+// the high-priority side stream and the ordering events kbk_cholesky needs for a matrix of n_pad rows (kept on the handle)
+static int cholesky_streams(kb200_ctx* h, int n_pad) {
+    if (!h->hi_stream) {
+        int lo = 0, hi = 0;
+        CU(h, cudaDeviceGetStreamPriorityRange(&lo, &hi));
+        CU(h, cudaStreamCreateWithPriority(&h->hi_stream, cudaStreamNonBlocking, hi));
+    }
+    const size_t need = 2 * (size_t)((n_pad / 64 + 3) / 4) + 1;
+    while (h->fev.size() < need) {
+        cudaEvent_t e;
+        CU(h, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        h->fev.push_back(e);
+    }
+    return KB200_OK;
+}
+
 extern "C" int kb200_set_problem(kb200_handle h, int dim, int dtype, int64_t n,
                                  const double* x, const double* y, const double* z, const double* values,
                                  const double* center, const double* aniso,
@@ -655,17 +671,7 @@ extern "C" int kb200_set_problem(kb200_handle h, int dim, int dtype, int64_t n,
             t_asm += ev_ms(h->ev[EV_ASM], h->ev[EV_FACTOR]);
             break;
         }
-        if (!h->hi_stream) {
-            int lo = 0, hi = 0;
-            CU(h, cudaDeviceGetStreamPriorityRange(&lo, &hi));
-            CU(h, cudaStreamCreateWithPriority(&h->hi_stream, cudaStreamNonBlocking, hi));
-        }
-        const size_t need = 2 * (size_t)((np / 64 + 3) / 4) + 1;
-        while (h->fev.size() < need) {
-            cudaEvent_t e;
-            CU(h, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-            h->fev.push_back(e);
-        }
+        rc = cholesky_streams(h, np); if (rc) return rc;
         CU(h, kbk_cholesky(h->wC.as<double>(), h->wW.as<double>(), h->wT.as<double>(), ld, np, flag, 3.6e-15 * h->vg.c0, st, h->hi_stream,
                            h->fev.data(), (int)h->fev.size(), &launches));
         CU(h, cudaEventRecord(h->ev[EV_INVERT], st));
@@ -997,7 +1003,9 @@ extern "C" int kb200_set_problem_knn(kb200_handle h, int dim, int64_t n,
     return KB200_OK;
 }
 
-static int run_knn(kb200_ctx* h, int k, const Src& s, double* d_z, double* d_ss, int chol, int loo) {
+// mode, sg, qg: kbk_knn_solve's mode and group arrays (1: leave-one-out, 2: leave-group-out of the stations)
+static int run_knn(kb200_ctx* h, int k, const Src& s, double* d_z, double* d_ss, int chol, int mode = 0,
+                   const int* sg = nullptr, const int* qg = nullptr) {
     cudaStream_t st = h->stream;
     KnnParams kp = h->kp;
     kp.vg = h->vg; kp.an = h->an; kp.k = k;
@@ -1010,8 +1018,7 @@ static int run_knn(kb200_ctx* h, int k, const Src& s, double* d_z, double* d_ss,
         kp.r0 = (int)std::min(64.0, std::max(1.0, std::ceil(R)));
     }
     kp.ps = s.point_source(); kp.m = s.count; kp.z_out = d_z; kp.ss_out = d_ss; kp.flag = h->wFlag.as<int>(); kp.zstride = h->zstride;
-    if (loo == 2) CU(h, kbk_knn_solve_lgo(kp, chol, h->lgo_sg, h->lgo_qg, st));
-    else CU(h, kbk_knn_solve(kp, chol, st, loo));
+    CU(h, kbk_knn_solve(kp, chol, st, mode, sg, qg));
     h->launches += 1; h->solve_launches += 1;
     return KB200_OK;
 }
@@ -1046,10 +1053,11 @@ static int knn_retry(kb200_ctx* h, Run run) {
     return KB200_OK;
 }
 
-static int knn_to_host(kb200_ctx* h, int k, const Src& s, double* z_out, double* ss_out, int loo) {
+static int knn_to_host(kb200_ctx* h, int k, const Src& s, double* z_out, double* ss_out, int mode = 0,
+                       const int* sg = nullptr, const int* qg = nullptr) {
     return knn_retry(h, [&](int chol) {
         return run_to_host(h, s.count, z_out, ss_out, [&](int64_t o, int64_t c, double* dz, double* dss) {
-            return run_knn(h, k, s.sub(o, c), dz, dss, chol, loo);
+            return run_knn(h, k, s.sub(o, c), dz, dss, chol, mode, sg, qg);
         });
     });
 }
@@ -1065,7 +1073,7 @@ extern "C" int kb200_execute_knn_grid_dev(kb200_handle h, int k, int64_t nx, int
     h->zstride = count;
     return knn_retry(h, [&](int chol) {
         CU(h, cudaEventRecord(h->ev[EV_RUN], h->stream));
-        int rc = run_knn(h, k, s, d_z, d_ss, chol, 0); if (rc) return rc;
+        int rc = run_knn(h, k, s, d_z, d_ss, chol); if (rc) return rc;
         CU(h, cudaEventRecord(h->ev[EV_RUN_END], h->stream));
         return KB200_OK;
     });
@@ -1122,7 +1130,7 @@ static int exec_host(kb200_ctx* h, bool knn, int k, const Query& q, double* z_ou
     Src s{};
     rc = upload_query(h, q, &s); if (rc) return rc;
     const int64_t off = q.first - q.cfirst;
-    rc = knn ? knn_to_host(h, k, s, z_out + off, ss_out + off, 0)
+    rc = knn ? knn_to_host(h, k, s, z_out + off, ss_out + off)
              : run_to_host(h, q.count, z_out + off, ss_out + off, [&](int64_t o, int64_t c, double* dz, double* dss) {
                    return run_solve(h, s.sub(o, c), dz, dss);
                });
@@ -1423,60 +1431,81 @@ extern "C" int64_t kb200_debug_fetch(kb200_handle h, int what, double* out, int6
 // drift block is singular (e.g. universal kriging with n - 1 < K + 1 stations, or the rest collinear for a linear drift)
 static const double KB_LOO_TOL = 1e-10;
 
-extern "C" int kb200_loo(kb200_handle h, double* z_out, double* ss_out) {
+// the preconditions of the global cross-validation paths; what ("leave-one-out", "leave-group-out") names the feature
+static int check_cv(kb200_ctx* h, const double* z_out, const double* ss_out, const char* what) {
     if (!h || !z_out || !ss_out) return KB200_EBADARG;
     if (!h->ready) return fail(h, KB200_ESTATE, "no factored problem: call kb200_set_problem first");
-    if (h->gform == 2) return fail(h, KB200_EUNSUPPORTED, "leave-one-out needs the inverse of the kriging matrix; "
+    if (h->gform == 2) return fail(h, KB200_EUNSUPPORTED, std::string(what) + " needs the inverse of the kriging matrix; "
                                    "the pseudo-inverse (pseudo_inv=True) does not give it");
     if (!h->local_factor) return fail(h, KB200_ESTATE, "the factorisation is not on this handle "
                                       "(problem received through kb200_blob_commit)");
+    return KB200_OK;
+}
+
+// exact_values: the stations j != i within eps of every station i (grp, a device array: only those of another group),
+// ascending j. The lists stay on the device (h->wPairs), station i's at pj/pd + off[i], and st lists the stations that
+// have any. Only the counts come to the host, where more than LOO_MAXDUP for one station refuse the call.
+struct NearPairs {
+    std::vector<int> cnt, hoff, st;            // host: count and list offset of every station, the stations with near
+                                               // pairs (ascending)
+    const int* d_st = nullptr; const int* off = nullptr; const int* pj = nullptr; const double* pd = nullptr;
+};
+static int near_pairs(kb200_ctx* h, const int* grp, const char* what, const char* others, NearPairs& np, int* launches) {
+    cudaStream_t st = h->stream;
+    const int nn = h->n;
+    const BlobView b = blob_view(h);
+    // ints: cnt [n] | off [n + 1] | st [n], then doubles: pd, then ints: pj
+    const size_t pd_at = align_up((3 * (size_t)nn + 1) * sizeof(int), sizeof(double));
+    CU(h, h->wPairs.reserve(pd_at));
+    int* cnt = h->wPairs.as<int>();
+    CU(h, kbk_loo_pairs(h->dim, nn, b.ax, b.ay, b.az, h->vg.eps, grp, cnt, nullptr, nullptr, nullptr, st)); ++*launches;
+    np.cnt.resize(nn);
+    CU(h, cudaMemcpyAsync(np.cnt.data(), cnt, (size_t)nn * sizeof(int), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    std::vector<int>& hoff = np.hoff;
+    hoff.assign(nn + 1, 0);
+    for (int i = 0; i < nn; ++i) {
+        if (np.cnt[i] > LOO_MAXDUP)
+            return fail(h, KB200_EUNSUPPORTED, std::string(what) + ": station " + std::to_string(i) + " has " +
+                        std::to_string(np.cnt[i]) + " " + others + " within eps (at most " + std::to_string(LOO_MAXDUP) + ")");
+        hoff[i + 1] = hoff[i] + np.cnt[i];
+        if (np.cnt[i]) np.st.push_back(i);
+    }
+    if (np.st.empty()) return KB200_OK;
+    const size_t tot = (size_t)hoff[nn];
+    CU(h, h->wPairs.reserve(pd_at + tot * (sizeof(double) + sizeof(int))));      // the counts are on the host now
+    int* off = h->wPairs.as<int>() + nn;
+    int* dst = off + nn + 1;
+    double* pd = reinterpret_cast<double*>(h->wPairs.as<char>() + pd_at);
+    int* pj = reinterpret_cast<int*>(pd + tot);
+    CU(h, cudaMemcpyAsync(off, hoff.data(), (size_t)(nn + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
+    CU(h, cudaMemcpyAsync(dst, np.st.data(), np.st.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    CU(h, kbk_loo_pairs(h->dim, nn, b.ax, b.ay, b.az, h->vg.eps, grp, nullptr, off, pj, pd, st)); ++*launches;
+    np.d_st = dst; np.off = off; np.pj = pj; np.pd = pd;
+    return KB200_OK;
+}
+
+extern "C" int kb200_loo(kb200_handle h, double* z_out, double* ss_out) {
+    int rc = check_cv(h, z_out, ss_out, "leave-one-out"); if (rc) return rc;
     cudaSetDevice(h->device);
     cudaStream_t st = h->stream;
     const int nn = h->n, np = h->n_pad, nv = h->nf ? h->nf : 1;
     const int nch = (nn + LOO_RC - 1) / LOO_RC;
-    // doubles: part [nch][n] | pii [n] | alpha [nv][n] | z [nv][n] | ss [n], then ints: cnt [n] | off [n + 1] | st [n] | bad
-    const size_t nd = ((size_t)nch + 2 + 2 * (size_t)nv) * nn, ni = 3 * (size_t)nn + 2;
-    CU(h, h->wLoo.reserve(nd * sizeof(double) + ni * sizeof(int)));
+    // doubles: part [nch][n] | pii [n] | alpha [nv][n] | z [nv][n] | ss [n], then the int bad
+    const size_t nd = ((size_t)nch + 2 + 2 * (size_t)nv) * nn;
+    CU(h, h->wLoo.reserve(nd * sizeof(double) + sizeof(int)));
     double* part = h->wLoo.as<double>();
     double* pii = part + (size_t)nch * nn;
     double* alpha = pii + nn;
     double* dz = alpha + (size_t)nv * nn;
     double* dss = dz + (size_t)nv * nn;
-    int* cnt = reinterpret_cast<int*>(h->wLoo.as<double>() + nd);
-    int* off = cnt + nn;
-    int* slist = off + nn + 1;
-    int* bad = slist + nn;
+    int* bad = reinterpret_cast<int*>(h->wLoo.as<double>() + nd);
     const BlobView b = blob_view(h);
     int launches = 0;
+    NearPairs dup;
+    if (h->vg.exact) { rc = near_pairs(h, nullptr, "leave-one-out", "other stations", dup, &launches); if (rc) return rc; }
 
-    // exact_values: stations within eps of each other (counts, then the lists at host-scanned offsets)
-    std::vector<int> hcnt, hoff, hst;
-    int* pj = nullptr; double* pd = nullptr;
-    if (h->vg.exact) {
-        CU(h, kbk_loo_pairs(h->dim, nn, b.ax, b.ay, b.az, h->vg.eps, cnt, nullptr, nullptr, nullptr, st)); ++launches;
-        hcnt.resize(nn);
-        CU(h, cudaMemcpyAsync(hcnt.data(), cnt, (size_t)nn * sizeof(int), cudaMemcpyDeviceToHost, st));
-        CU(h, cudaStreamSynchronize(st));
-        hoff.assign(nn + 1, 0);
-        for (int i = 0; i < nn; ++i) {
-            if (hcnt[i] > LOO_MAXDUP)
-                return fail(h, KB200_EUNSUPPORTED, "leave-one-out: station " + std::to_string(i) + " has " +
-                            std::to_string(hcnt[i]) + " other stations within eps (at most " + std::to_string(LOO_MAXDUP) + ")");
-            hoff[i + 1] = hoff[i] + hcnt[i];
-            if (hcnt[i]) hst.push_back(i);
-        }
-        if (hoff[nn] > 0) {
-            const size_t tot = (size_t)hoff[nn];
-            CU(h, h->wVario.reserve(tot * (sizeof(double) + sizeof(int))));
-            pd = h->wVario.as<double>();
-            pj = reinterpret_cast<int*>(pd + tot);
-            CU(h, cudaMemcpyAsync(off, hoff.data(), (size_t)(nn + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
-            CU(h, cudaMemcpyAsync(slist, hst.data(), hst.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-            CU(h, kbk_loo_pairs(h->dim, nn, b.ax, b.ay, b.az, h->vg.eps, cnt, off, pj, pd, st)); ++launches;
-        }
-    }
-
-    LooParams p{};
+    CvParams p{};
     p.n = nn; p.n_pad = np; p.ld = h->ld; p.K1 = h->K1; p.nv = nv; p.gform = h->gform; p.nchunks = nch;
     p.tol = KB_LOO_TOL; p.vg = h->vg;
     p.W = h->wW.as<double>(); p.G = h->wC.as<double>(); p.part = part;
@@ -1489,7 +1518,9 @@ extern "C" int kb200_loo(kb200_handle h, double* z_out, double* ss_out) {
     CU(h, cudaEventRecord(h->ev[EV_RUN], st));
     if (h->gform == 0) { CU(h, kbk_loo_colsq(p.W, p.ld, nn, part, st)); ++launches; }
     CU(h, kbk_loo_finalize(p, st)); ++launches;
-    if (!hst.empty()) { CU(h, kbk_loo_dup(p, (int)hst.size(), slist, off, pj, pd, st)); ++launches; }
+    if (!dup.st.empty()) {
+        CU(h, kbk_loo_dup(p, (int)dup.st.size(), dup.d_st, dup.off, dup.pj, dup.pd, st)); ++launches;
+    }
     CU(h, cudaEventRecord(h->ev[EV_RUN_END], st));
     int hbad = big;
     CU(h, cudaMemcpyAsync(&hbad, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1504,13 +1535,16 @@ extern "C" int kb200_loo(kb200_handle h, double* z_out, double* ss_out) {
     return KB200_OK;
 }
 
+// the stations' raw coordinates as the query points of the moving-window cross-validation
+static Src station_queries(kb200_ctx* h) {
+    return Src{false, 0, 0, 0, raw_col(h, RAW_X), raw_col(h, RAW_Y), raw_col(h, RAW_Z), 0, h->n, nullptr, 0, 0};
+}
+
 extern "C" int kb200_knn_loo(kb200_handle h, int k, double* z_out, double* ss_out) {
     int rc = check_knn(h, k); if (rc) return rc;
     if (k > h->n - 1) return fail(h, KB200_EBADARG, "leave-one-out: n_closest_points must be at most n - 1");
     if (!z_out || !ss_out) return fail(h, KB200_EBADARG, "null pointer");
-    // the stations' raw coordinates are the query points
-    const Src s{false, 0, 0, 0, raw_col(h, RAW_X), raw_col(h, RAW_Y), raw_col(h, RAW_Z), 0, h->n, nullptr, 0, 0};
-    return knn_to_host(h, k, s, z_out, ss_out, 1);
+    return knn_to_host(h, k, station_queries(h), z_out, ss_out, 1);
 }
 
 // ---- leave-group-out cross-validation (DESIGN.md §5f) ---------------------------------------------------------------
@@ -1530,14 +1564,9 @@ static int check_groups(kb200_ctx* h, const int32_t* group, int n_groups, std::v
 }
 
 extern "C" int kb200_lgo(kb200_handle h, const int32_t* group, int n_groups, double* z_out, double* ss_out) {
-    if (!h || !z_out || !ss_out) return KB200_EBADARG;
-    if (!h->ready) return fail(h, KB200_ESTATE, "no factored problem: call kb200_set_problem first");
-    if (h->gform == 2) return fail(h, KB200_EUNSUPPORTED, "leave-group-out needs the inverse of the kriging matrix; "
-                                   "the pseudo-inverse (pseudo_inv=True) does not give it");
-    if (!h->local_factor) return fail(h, KB200_ESTATE, "the factorisation is not on this handle "
-                                      "(problem received through kb200_blob_commit)");
+    int rc = check_cv(h, z_out, ss_out, "leave-group-out"); if (rc) return rc;
     std::vector<int> sizes;
-    int rc = check_groups(h, group, n_groups, sizes); if (rc) return rc;
+    rc = check_groups(h, group, n_groups, sizes); if (rc) return rc;
     if (n_groups == h->n) return kb200_loo(h, z_out, ss_out);      // every group a singleton: leave-one-out
     cudaSetDevice(h->device);
     cudaStream_t st = h->stream;
@@ -1561,50 +1590,11 @@ extern "C" int kb200_lgo(kb200_handle h, const int32_t* group, int n_groups, dou
         else large.push_back(g);
     }
 
-    // exact_values: near pairs of stations in different groups (the pairs inside a group are held out together)
-    std::vector<int> dst, doff(1, 0), dj; std::vector<double> dd; std::vector<long long> soff(1, 0);
-    if (h->vg.exact) {
-        CU(h, h->wLoo.reserve((size_t)(2 * nn + 1) * sizeof(int)));
-        int* cnt = h->wLoo.as<int>();
-        int* off = cnt + nn;
-        CU(h, kbk_loo_pairs(h->dim, nn, b.ax, b.ay, b.az, h->vg.eps, cnt, nullptr, nullptr, nullptr, st)); ++launches;
-        std::vector<int> hcnt(nn), hoff(nn + 1, 0);
-        CU(h, cudaMemcpyAsync(hcnt.data(), cnt, (size_t)nn * sizeof(int), cudaMemcpyDeviceToHost, st));
-        CU(h, cudaStreamSynchronize(st));
-        for (int i = 0; i < nn; ++i) hoff[i + 1] = hoff[i] + hcnt[i];
-        if (hoff[nn] > 0) {
-            const size_t tot = (size_t)hoff[nn];
-            CU(h, h->wVario.reserve(tot * (sizeof(double) + sizeof(int))));
-            double* pd = h->wVario.as<double>();
-            int* pj = reinterpret_cast<int*>(pd + tot);
-            CU(h, cudaMemcpyAsync(off, hoff.data(), (size_t)(nn + 1) * sizeof(int), cudaMemcpyHostToDevice, st));
-            CU(h, kbk_loo_pairs(h->dim, nn, b.ax, b.ay, b.az, h->vg.eps, cnt, off, pj, pd, st)); ++launches;
-            std::vector<int> hpj(tot); std::vector<double> hpd(tot);
-            CU(h, cudaMemcpyAsync(hpj.data(), pj, tot * sizeof(int), cudaMemcpyDeviceToHost, st));
-            CU(h, cudaMemcpyAsync(hpd.data(), pd, tot * sizeof(double), cudaMemcpyDeviceToHost, st));
-            CU(h, cudaStreamSynchronize(st));
-            for (int i = 0; i < nn; ++i) {
-                int c = 0;
-                for (int t = hoff[i]; t < hoff[i + 1]; ++t)
-                    if (group[hpj[t]] != group[i]) { dj.push_back(hpj[t]); dd.push_back(hpd[t]); ++c; }
-                if (!c) continue;
-                if (c > LOO_MAXDUP)
-                    return fail(h, KB200_EUNSUPPORTED, "leave-group-out: station " + std::to_string(i) + " has " +
-                                std::to_string(c) + " stations of other groups within eps (at most " +
-                                std::to_string(LOO_MAXDUP) + ")");
-                dst.push_back(i); doff.push_back((int)dj.size());
-                soff.push_back(soff.back() + 2LL * c * sizes[group[i]]);
-            }
-        }
-    }
-    const int nst = (int)dst.size();
-
-    // workspace (doubles): blk | scale [n] | alpha [nv][n] | e [nv][n] | z [nv][n] | ss [n] | pii [n] |
-    // dd | dup scratch; then long long: boff | soff; then int: grp | mem | goff | pos | small | dst | doff | dj | bad
-    const size_t ndbl = (size_t)nblk + (size_t)nn * (3 + 3 * (size_t)nv) + dd.size() + (size_t)soff.back();
-    const size_t nll = boff.size() + soff.size();
-    const size_t nint = 3 * (size_t)nn + goff.size() + small.size() + dst.size() + doff.size() + dj.size() + 2;
-    CU(h, h->wLgo.reserve(ndbl * 8 + nll * 8 + nint * 4 + 256));
+    // workspace (doubles): blk | scale [n] | alpha [nv][n] | e [nv][n] | z [nv][n] | ss [n] | pii [n]; then long long:
+    // boff; then int: grp | mem | goff | pos | small | bad | the leave-one-out finalize's bad
+    const size_t ndbl = (size_t)nblk + (size_t)nn * (3 + 3 * (size_t)nv);
+    const size_t nint = 3 * (size_t)nn + goff.size() + small.size() + 2;
+    CU(h, h->wLgo.reserve(ndbl * 8 + boff.size() * 8 + nint * 4));
     double* blk = h->wLgo.as<double>();
     double* scale = blk + nblk;
     double* alpha = scale + nn;
@@ -1612,25 +1602,32 @@ extern "C" int kb200_lgo(kb200_handle h, const int32_t* group, int n_groups, dou
     double* dz = de + (size_t)nv * nn;
     double* dss = dz + (size_t)nv * nn;
     double* lpii = dss + nn;
-    double* ddd = lpii + nn;
-    double* dscr = ddd + dd.size();
-    long long* dboff = reinterpret_cast<long long*>(dscr + soff.back());
-    long long* dsoff = dboff + boff.size();
-    int* dgrp = reinterpret_cast<int*>(dsoff + soff.size());
+    long long* dboff = reinterpret_cast<long long*>(lpii + nn);
+    int* dgrp = reinterpret_cast<int*>(dboff + boff.size());
     int* dmem = dgrp + nn; int* dgoff = dmem + nn; int* dpos = dgoff + goff.size(); int* dsmall = dpos + nn;
-    int* ddst = dsmall + small.size(); int* ddoff = ddst + dst.size(); int* ddj = ddoff + doff.size();
-    int* bad = ddj + dj.size(); int* lbad = bad + 1;
+    int* bad = dsmall + small.size(); int* lbad = bad + 1;
     auto up = [&](void* d, const void* s, size_t bytes) {
         return bytes ? cudaMemcpyAsync(d, s, bytes, cudaMemcpyHostToDevice, st) : cudaSuccess;
     };
     CU(h, up(dgrp, group, (size_t)nn * 4)); CU(h, up(dmem, mem.data(), (size_t)nn * 4));
     CU(h, up(dgoff, goff.data(), goff.size() * 4)); CU(h, up(dpos, pos.data(), (size_t)nn * 4));
     CU(h, up(dsmall, small.data(), small.size() * 4)); CU(h, up(dboff, boff.data(), boff.size() * 8));
-    CU(h, up(ddst, dst.data(), dst.size() * 4)); CU(h, up(ddoff, doff.data(), doff.size() * 4));
-    CU(h, up(ddj, dj.data(), dj.size() * 4)); CU(h, up(ddd, dd.data(), dd.size() * 8));
-    CU(h, up(dsoff, soff.data(), soff.size() * 8));
     const int big = INT_MAX;
     CU(h, up(bad, &big, 4));
+
+    // exact_values: near pairs of stations in different groups (the pairs inside a group are held out together), and
+    // in wLoo (free during this call) the correction's scratch of each such station: soff | P_jS and P_jS Q (|D| x m)
+    NearPairs dup;
+    if (h->vg.exact) {
+        rc = near_pairs(h, dgrp, "leave-group-out", "stations of other groups", dup, &launches); if (rc) return rc;
+    }
+    const int nst = (int)dup.st.size();
+    std::vector<long long> soff(1, 0);
+    for (int i : dup.st) soff.push_back(soff.back() + 2LL * dup.cnt[i] * sizes[group[i]]);
+    CU(h, h->wLoo.reserve((soff.size() + (size_t)soff.back()) * 8));
+    long long* dsoff = h->wLoo.as<long long>();
+    double* dscr = reinterpret_cast<double*>(dsoff + soff.size());
+    CU(h, up(dsoff, soff.data(), soff.size() * 8));
 
     // G = C^-1: W^T W into wT (free after kb200_set_problem), or the Gauss-Jordan inverse already in wC
     CU(h, cudaEventRecord(h->ev[EV_RUN], st));
@@ -1640,17 +1637,16 @@ extern "C" int kb200_lgo(kb200_handle h, const int32_t* group, int n_groups, dou
         G = h->wT.as<double>();
     }
     CU(h, cudaEventRecord(h->ev[EV_INVERT], st));
-    // alpha_v = P Z_v: the leave-one-out finalize on G (its other outputs are overwritten below)
-    LooParams lp{};
-    lp.n = nn; lp.n_pad = np; lp.ld = ld; lp.K1 = h->K1; lp.nv = nv; lp.gform = 1; lp.nchunks = 0;
-    lp.tol = KB_LOO_TOL; lp.vg = h->vg; lp.G = G; lp.Uz = aux_block(h, AUX_U); lp.consts = b.consts;
-    lp.Z = kriged_values(h); lp.pii = lpii; lp.alpha = alpha; lp.z_out = dz; lp.ss_out = dss; lp.bad = lbad;
-    LgoParams p{};
-    p.n = nn; p.n_pad = np; p.ld = ld; p.K1 = h->K1; p.nv = nv; p.tol = KB_LOO_TOL; p.vg = h->vg;
-    p.G = G; p.Uz = lp.Uz; p.consts = b.consts; p.Z = lp.Z; p.alpha = alpha;
+    CvParams p{};
+    p.n = nn; p.n_pad = np; p.ld = ld; p.K1 = h->K1; p.nv = nv; p.gform = 1; p.nchunks = 0;
+    p.tol = KB_LOO_TOL; p.vg = h->vg; p.G = G; p.Uz = aux_block(h, AUX_U); p.consts = b.consts;
+    p.Z = kriged_values(h); p.pii = lpii; p.alpha = alpha;
     p.grp = dgrp; p.mem = dmem; p.goff = dgoff; p.pos = dpos; p.boff = dboff; p.blk = blk; p.scale = scale; p.e = de;
-    p.z_out = dz; p.ss_out = dss; p.bad = bad;
-    CU(h, kbk_loo_finalize(lp, st)); ++launches;
+    p.z_out = dz; p.ss_out = dss; p.bad = lbad;
+    // alpha_v = P Z_v: the leave-one-out finalize on G (its other outputs are overwritten below, and a station whose
+    // P_ii is at rounding level, lbad, is no refusal of its group)
+    CU(h, kbk_loo_finalize(p, st)); ++launches;
+    p.bad = bad;
     CU(h, kbk_lgo_gather(p, n_groups, max_m, st)); ++launches;
     CU(h, kbk_lgo_small(p, (int)small.size(), dsmall, max_small, st)); launches += small.empty() ? 0 : 1;
 
@@ -1669,17 +1665,7 @@ extern "C" int kb200_lgo(kb200_handle h, const int32_t* group, int n_groups, dou
         double* T1 = Wm + mat;
         int* flag = reinterpret_cast<int*>(T1 + mat);
         if (h->gform == 1) CU(h, h->wVario.reserve(kbk_general_inverse_workspace_bytes(mp)));
-        if (!h->hi_stream) {
-            int lo = 0, hi = 0;
-            CU(h, cudaDeviceGetStreamPriorityRange(&lo, &hi));
-            CU(h, cudaStreamCreateWithPriority(&h->hi_stream, cudaStreamNonBlocking, hi));
-        }
-        const size_t need = 2 * (size_t)((mp / 64 + 3) / 4) + 1;
-        while (h->fev.size() < need) {
-            cudaEvent_t e;
-            CU(h, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-            h->fev.push_back(e);
-        }
+        rc = cholesky_streams(h, mp); if (rc) return rc;
         for (int g : large) {
             const int m = sizes[g], gp = (int)align_up((size_t)m, 64);
             double smax = 0.0;
@@ -1704,7 +1690,7 @@ extern "C" int kb200_lgo(kb200_handle h, const int32_t* group, int n_groups, dou
     }
     CU(h, cudaEventRecord(h->ev[EV_DUAL], st));
     CU(h, kbk_lgo_finalize(p, st)); ++launches;
-    if (nst) { CU(h, kbk_lgo_dup(p, nst, ddst, ddoff, ddj, ddd, dsoff, dscr, st)); ++launches; }
+    if (nst) { CU(h, kbk_lgo_dup(p, nst, dup.d_st, dup.off, dup.pj, dup.pd, dsoff, dscr, st)); ++launches; }
     CU(h, cudaEventRecord(h->ev[EV_RUN_END], st));
     int hbad = big;
     CU(h, cudaMemcpyAsync(&hbad, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1739,9 +1725,5 @@ extern "C" int kb200_knn_lgo(kb200_handle h, int k, const int32_t* group, int n_
     CU(h, cudaMemcpyAsync(qg, group, (size_t)nn * sizeof(int), cudaMemcpyHostToDevice, h->stream));
     CU(h, kbk_knn_sort_groups(nn, sorig, qg, sg, h->stream));
     h->launches += 1;
-    h->lgo_sg = sg; h->lgo_qg = qg;
-    const Src s{false, 0, 0, 0, raw_col(h, RAW_X), raw_col(h, RAW_Y), raw_col(h, RAW_Z), 0, h->n, nullptr, 0, 0};
-    rc = knn_to_host(h, k, s, z_out, ss_out, 2);
-    h->lgo_sg = nullptr; h->lgo_qg = nullptr;
-    return rc;
+    return knn_to_host(h, k, station_queries(h), z_out, ss_out, 2, sg, qg);
 }

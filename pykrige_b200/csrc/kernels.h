@@ -284,12 +284,11 @@ struct KnnParams {
 cudaError_t kbk_knn_build(int dim, int n, const double* ax, const double* ay, const double* az, const double* values,
                           KnnParams& kp, double* sx, double* sy, double* sz, double* sv, int* sorig,
                           int* cell_of, int* cell_start, int* cursor, int ncells, cudaStream_t st, int* launches);
-// loo = 1: leave-one-out of every station, query p = station ps.first + p (ps = the raw station coordinates), and the
-// candidate with that original index is never counted
-cudaError_t kbk_knn_solve(const KnnParams& p, int chol, cudaStream_t st, int loo = 0);
-// leave-group-out: as loo = 1, but every candidate whose group (sgroup, cell-sorted) equals the query station's group
-// (qgroup, original order) is never counted
-cudaError_t kbk_knn_solve_lgo(const KnnParams& p, int chol, const int* sgroup, const int* qgroup, cudaStream_t st);
+// mode 1: leave-one-out of every station, query p = station ps.first + p (ps = the raw station coordinates), and the
+// candidate with that original index is never counted; mode 2: leave-group-out, as mode 1, but every candidate whose
+// group (sgroup, cell-sorted) equals the query station's group (qgroup, original order) is never counted
+cudaError_t kbk_knn_solve(const KnnParams& p, int chol, cudaStream_t st, int mode = 0, const int* sgroup = nullptr,
+                          const int* qgroup = nullptr);
 // dst[s] = src[sorig[s]]: group labels in the cell-sorted order of the moving window
 cudaError_t kbk_knn_sort_groups(int n, const int* sorig, const int* src, int* dst, cudaStream_t st);
 size_t      kbk_knn_smem_per_warp(int k, int chol, int hasz, int nv);
@@ -310,42 +309,24 @@ cudaError_t kbk_statistics(int dim, int n, const double* ax, const double* ay, c
                            const double* L, int ld, const double* u, const double* zeta, int* dup,
                            double* delta, double* sigma, cudaStream_t st);
 
-// loo.cu: leave-one-out cross-validation of every station from the held factorisation (DESIGN.md §5e)
+// loo.cu: leave-one-out (DESIGN.md §5e) and leave-group-out (§5f) cross-validation from the held factorisation
 #define LOO_RC 256          // rows per chunk of the column sums of squares of W
 #define LOO_MAXDUP 32       // stations within eps of one station that the exact-hit correction handles
-struct LooParams {
-    int n, n_pad, ld, K1, nv, gform, nchunks;
-    double tol;                // |P_ii| <= tol * max(|diag term|, |u_i^T S^-1 u_i|): drift not determined without i
+#define LGO_SMALL 128       // largest group whose block is inverted in shared memory (one CTA); larger: blocked kernels
+struct CvParams {
+    int n, n_pad, ld, K1, nv;
+    int gform, nchunks;        // leave-one-out finalize: 0 reads W's column sums, 1 reads G
+    double tol;                // leave-one-out: |P_ii| <= tol * max(|diag term|, |u_i^T S^-1 u_i|): drift not determined
+                               // without i; leave-group-out: the same bound on a pivot against the scale of its station
     VgParams vg;
     const double* W;           // gform 0: W = L^-1 (lower triangle, row-major, ld)
-    const double* G;           // gform 1: G = C^-1 (full, row-major, ld)
+    const double* G;           // gform 1: G = C^-1 (row-major, ld; full for leave-one-out, lower triangle for leave-group-out)
     const double* part;        // gform 0: [nchunks][n] chunk sums of squares of W's columns
     const double* Uz;          // [K1 + nv][n_pad]: U = C^-1 F (rescaled drift + ones), then zeta_v = C^-1 Z_v
     const double* consts;      // S^-1 (K1 x K1), then phi_v (K1 each)
     const double* Z;           // [nv][n] station values
-    double* pii; double* alpha;   // [n], [nv][n]: kept for the exact-hit correction
-    double* z_out; double* ss_out;   // [nv][n], [n]
-    int* bad;                  // lowest station whose P_ii is at rounding level (INT_MAX: none)
-};
-cudaError_t kbk_loo_colsq(const double* W, int ld, int n, double* part, cudaStream_t st);
-cudaError_t kbk_loo_finalize(const LooParams& p, cudaStream_t st);
-// off == NULL: cnt[i] = |D(i)|; else station i's near stations j (ascending) and distances at pj/pd + off[i]
-cudaError_t kbk_loo_pairs(int dim, int n, const double* ax, const double* ay, const double* az, double eps, int* cnt,
-                          const int* off, int* pj, double* pd, cudaStream_t st);
-cudaError_t kbk_loo_dup(const LooParams& p, int nst, const int* st_list, const int* off, const int* pj, const double* pd,
-                        cudaStream_t st);
-
-// loo.cu: leave-group-out cross-validation (DESIGN.md §5f)
-#define LGO_SMALL 128       // largest group whose block is inverted in shared memory (one CTA); larger: blocked kernels
-struct LgoParams {
-    int n, n_pad, ld, K1, nv;
-    double tol;                // a pivot at or below tol * scale of its station: drift not determined without the group
-    VgParams vg;
-    const double* G;           // G = C^-1, lower triangle (row-major, ld)
-    const double* Uz;          // as LooParams
-    const double* consts;
-    const double* Z;
-    const double* alpha;       // [nv][n] alpha_v = P Z_v (loo_finalize_kernel)
+    double* pii; double* alpha;   // [n], [nv][n] alpha_v = P Z_v: kept for the exact-hit corrections
+    // leave-group-out only
     const int* grp;            // [n] dense group index of each station
     const int* mem;            // [n] the stations group by group, ascending inside a group
     const int* goff;           // [n_groups + 1] group g is mem[goff[g] .. goff[g + 1])
@@ -355,18 +336,28 @@ struct LgoParams {
     double* scale;             // [n] in mem order: max(|G_ii|, |u_i^T S^-1 u_i|)
     double* e;                 // [nv][n] e_S,v of each station
     double* z_out; double* ss_out;   // [nv][n], [n]
-    int* bad;                  // lowest group whose block has a pivot at rounding level (INT_MAX: none)
+    int* bad;                  // leave-one-out: lowest station whose P_ii is at rounding level; leave-group-out: lowest
+                               // group whose block has a pivot at rounding level (INT_MAX: none)
 };
+cudaError_t kbk_loo_colsq(const double* W, int ld, int n, double* part, cudaStream_t st);
+cudaError_t kbk_loo_finalize(const CvParams& p, cudaStream_t st);
+// near stations j != i within eps of every station i (grp != NULL: only those with grp[j] != grp[i]), ascending j:
+// off == NULL: cnt[i] = their count; else their indices and distances at pj/pd + off[i]
+cudaError_t kbk_loo_pairs(int dim, int n, const double* ax, const double* ay, const double* az, double eps,
+                          const int* grp, int* cnt, const int* off, int* pj, double* pd, cudaStream_t st);
+// the exact-hit corrections: one warp per station i of st_list, its near stations at pj/pd + off[i] (off: [n + 1])
+cudaError_t kbk_loo_dup(const CvParams& p, int nst, const int* st_list, const int* off, const int* pj, const double* pd,
+                        cudaStream_t st);
 // G = W^T W, lower tiles only (factor.cu, DMMA)
 cudaError_t kbk_gram_lower(const double* W, int ld, int n_pad, double* G, int ldg, cudaStream_t st);
-cudaError_t kbk_lgo_gather(const LgoParams& p, int n_groups, int max_m, cudaStream_t st);
+cudaError_t kbk_lgo_gather(const CvParams& p, int n_groups, int max_m, cudaStream_t st);
 size_t      kbk_lgo_small_smem(int m);
-cudaError_t kbk_lgo_small(const LgoParams& p, int count, const int* glist, int max_m, cudaStream_t st);
+cudaError_t kbk_lgo_small(const CvParams& p, int count, const int* glist, int max_m, cudaStream_t st);
 cudaError_t kbk_lgo_pad(const double* blk, int m, double* dst, int ld, double d, cudaStream_t st);   // d: padding diagonal
 cudaError_t kbk_lgo_unpad(const double* src, int ld, double* blk, int m, cudaStream_t st);
-cudaError_t kbk_lgo_finalize(const LgoParams& p, cudaStream_t st);
-// one warp per station of st_list; its near stations of other groups at pj/pd + off[w] (off: [nst + 1])
-cudaError_t kbk_lgo_dup(const LgoParams& p, int nst, const int* st_list, const int* off, const int* pj, const double* pd,
+cudaError_t kbk_lgo_finalize(const CvParams& p, cudaStream_t st);
+// soff: [nst] start of each listed station's scratch (2 |D(i)| m doubles)
+cudaError_t kbk_lgo_dup(const CvParams& p, int nst, const int* st_list, const int* off, const int* pj, const double* pd,
                         const long long* soff, double* scratch, cudaStream_t st);
 
 // pinv.cu: pseudo_inv=True (one-sided Jacobi SVD of the bordered kriging matrix)

@@ -712,40 +712,25 @@ cudaError_t kbk_knn_sort_fields(int n, int nv, const int* sorig, const double* s
     return cudaGetLastError();
 }
 
-cudaError_t kbk_knn_solve(const KnnParams& p, int chol, cudaStream_t st, int loo) {
+cudaError_t kbk_knn_solve(const KnnParams& p, int chol, cudaStream_t st, int mode, const int* sgroup, const int* qgroup) {
     return KbDims::dispatch(p.dim, [&](auto D) {
         return KbModels::dispatch(p.vg.model, [&](auto M) {
             return KbBools::dispatch(chol && p.k <= 128, [&](auto CHOL) {
-                return KbBools::dispatch(loo != 0, [&](auto LOO) {
+                return KbList<0, 1, 2>::dispatch(mode, [&](auto MODE) {
                     const size_t per = kbk_knn_smem_per_warp(p.k, CHOL, KB_HASZ(D) ? 1 : 0, p.nv);
                     // as many points in flight per SM as fit (<= 320 threads; 227 KB minus the static 1 KB)
                     const int wpc = (int)std::min<size_t>(10, (size_t)(226 * 1024) / per);
                     if (wpc < 1) return cudaErrorInvalidValue;
                     const size_t smem = per * wpc;
-                    KB_CUDA_OK(cudaFuncSetAttribute(knn_solve_kernel<D, M, bool(CHOL), bool(LOO)>,
-                                                    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                    knn_solve_kernel<D, M, bool(CHOL), bool(LOO)><<<(unsigned)((p.m + wpc - 1) / wpc), wpc * 32, smem, st>>>(
-                        p, wpc, (int)(per / sizeof(double)));
-                    return cudaGetLastError();
+                    auto launch = [&](auto kernel, auto... groups) {
+                        KB_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                        kernel<<<(unsigned)((p.m + wpc - 1) / wpc), wpc * 32, smem, st>>>(p, wpc, (int)(per / sizeof(double)),
+                                                                                          groups...);
+                        return cudaGetLastError();
+                    };
+                    if constexpr (MODE == 2) return launch(knn_lgo_kernel<D, M, bool(CHOL)>, sgroup, qgroup);
+                    else return launch(knn_solve_kernel<D, M, bool(CHOL), MODE == 1>);
                 });
-            });
-        });
-    });
-}
-
-cudaError_t kbk_knn_solve_lgo(const KnnParams& p, int chol, const int* sgroup, const int* qgroup, cudaStream_t st) {
-    return KbDims::dispatch(p.dim, [&](auto D) {
-        return KbModels::dispatch(p.vg.model, [&](auto M) {
-            return KbBools::dispatch(chol && p.k <= 128, [&](auto CHOL) {
-                const size_t per = kbk_knn_smem_per_warp(p.k, CHOL, KB_HASZ(D) ? 1 : 0, p.nv);
-                const int wpc = (int)std::min<size_t>(10, (size_t)(226 * 1024) / per);
-                if (wpc < 1) return cudaErrorInvalidValue;
-                const size_t smem = per * wpc;
-                KB_CUDA_OK(cudaFuncSetAttribute(knn_lgo_kernel<D, M, bool(CHOL)>,
-                                                cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                knn_lgo_kernel<D, M, bool(CHOL)><<<(unsigned)((p.m + wpc - 1) / wpc), wpc * 32, smem, st>>>(
-                    p, wpc, (int)(per / sizeof(double)), sgroup, qgroup);
-                return cudaGetLastError();
             });
         });
     });

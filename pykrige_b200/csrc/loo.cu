@@ -37,7 +37,7 @@ __global__ void __launch_bounds__(LOO_CB) loo_colsq_kernel(const double* __restr
 
 // One thread per station: the diagonal term (chunk sums in chunk order, or G_ii), u_i^T S^-1 u_i, alpha_iv and the
 // outputs. Every product and sum of field v is the same whatever nv is and wherever v sits.
-__global__ void loo_finalize_kernel(LooParams P) {
+__global__ void loo_finalize_kernel(CvParams P) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= P.n) return;
     const int K1 = P.K1;
@@ -74,16 +74,20 @@ __global__ void loo_finalize_kernel(LooParams P) {
 }
 
 // Near pairs for exact_values: every j != i with |d_ij| <= eps, d as the solve kernels compute it for a data point and
-// a prediction point (adjusted coordinates; great-circle degrees for geographic). One thread per station i walks all j
-// in ascending order through shared-memory tiles: pass 0 counts, pass 1 writes station i's list at off[i] in j order.
-template <int DIM>
+// a prediction point (adjusted coordinates; great-circle degrees for geographic); with grp (leave-group-out) only the j
+// of another group than i. One thread per station i walks all j in ascending order through shared-memory tiles: pass 0
+// counts, pass 1 writes station i's list at off[i] in j order. GRP: grp is non-null (a template argument, so that the
+// leave-one-out scan keeps its loop).
+template <int DIM, bool GRP>
 __global__ void __launch_bounds__(256) loo_pairs_kernel(int n, const double* __restrict__ ax, const double* __restrict__ ay,
-                                                        const double* __restrict__ az, double eps, int* __restrict__ cnt,
+                                                        const double* __restrict__ az, double eps,
+                                                        const int* __restrict__ grp, int* __restrict__ cnt,
                                                         const int* __restrict__ off, int* __restrict__ pj,
                                                         double* __restrict__ pd) {
     __shared__ double sx[256], sy[256], sz[256];
     const int i = blockIdx.x * 256 + threadIdx.x;
     const double xi = i < n ? ax[i] : 0.0, yi = i < n ? ay[i] : 0.0, zi = i < n ? az[i] : 0.0;
+    const int gi = (GRP && i < n) ? grp[i] : 0;
     int c = 0;
     const int o = (off && i < n) ? off[i] : 0;
     for (int j0 = 0; j0 < n; j0 += 256) {
@@ -97,13 +101,31 @@ __global__ void __launch_bounds__(256) loo_pairs_kernel(int n, const double* __r
             const int j = j0 + q;
             if (j == i) continue;
             const double d = kb_dist<DIM>(sx[q], sy[q], sz[q], xi, yi, zi);     // (data j, prediction point i)
-            if (fabs(d) <= eps) {
+            if (fabs(d) <= eps && !(GRP && grp[j] == gi)) {
                 if (off) { pj[o + c] = j; pd[o + c] = d; }
                 ++c;
             }
         }
     }
     if (i < n && !off) cnt[i] = c;
+}
+
+// u_j^T S^-1 u_l (U: the first K1 columns of Uz, S^-1: the first K1 x K1 constants)
+__device__ double cv_usu(const CvParams& P, int j, int l) {
+    const int K1 = P.K1;
+    double usu = 0.0;
+    for (int a = 0; a < K1; ++a) {
+        double t = 0.0;
+        for (int b = 0; b < K1; ++b) t += P.consts[a * K1 + b] * P.Uz[(size_t)b * P.n_pad + l];
+        usu += P.Uz[(size_t)a * P.n_pad + j] * t;
+    }
+    return usu;
+}
+
+// sum over the 32 lanes of a warp by a fixed xor tree (every lane gets the same bits)
+__device__ __forceinline__ double cv_warp_sum(double s) {
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    return s;
 }
 
 __device__ double loo_gamma(const VgParams& v, double d) {
@@ -120,30 +142,23 @@ __device__ double loo_gamma(const VgParams& v, double d) {
 
 // P_jl by one warp: W[:, j] . W[:, l] over rows >= max(j, l) (lanes over rows, fixed xor tree), minus u_j^T S^-1 u_l;
 // gform 1: G_jl - u_j^T S^-1 u_l.
-__device__ double loo_pjl(const LooParams& P, int j, int l, int lane) {
+__device__ double loo_pjl(const CvParams& P, int j, int l, int lane) {
     double s;
     if (P.gform == 1) {
         s = P.G[(size_t)j * P.ld + l];
     } else {
         s = 0.0;
         for (int r = max(j, l) + lane; r < P.n; r += 32) s = fma(P.W[(size_t)r * P.ld + j], P.W[(size_t)r * P.ld + l], s);
-        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+        s = cv_warp_sum(s);
     }
-    const int K1 = P.K1;
-    double usu = 0.0;
-    for (int a = 0; a < K1; ++a) {
-        double t = 0.0;
-        for (int b = 0; b < K1; ++b) t += P.consts[a * K1 + b] * P.Uz[(size_t)b * P.n_pad + l];
-        usu += P.Uz[(size_t)a * P.n_pad + j] * t;
-    }
-    return s - usu;
+    return s - cv_usu(P, j, l);
 }
 
 // Exact-hit correction of station i (one warp per station that has near pairs), D = D(i), Delta_j = gamma(d_ij):
 //     zhat_v  += sum_j Delta_j (alpha_jv - alpha_iv P_ij / P_ii)
 //     sigma^2 += 2 sum_j Delta_j P_ij / P_ii - sum_{j,l} Delta_j Delta_l (P_jl - P_ij P_il / P_ii)
 // m = |D(i)| <= LOO_MAXDUP (the host checks); sums run in list order (ascending j).
-__global__ void __launch_bounds__(256) loo_dup_kernel(LooParams P, int nst, const int* __restrict__ st,
+__global__ void __launch_bounds__(256) loo_dup_kernel(CvParams P, int nst, const int* __restrict__ st,
                                                       const int* __restrict__ off, const int* __restrict__ pj,
                                                       const double* __restrict__ pd) {
     const int w = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
@@ -180,20 +195,22 @@ cudaError_t kbk_loo_colsq(const double* W, int ld, int n, double* part, cudaStre
     return cudaGetLastError();
 }
 
-cudaError_t kbk_loo_finalize(const LooParams& p, cudaStream_t st) {
+cudaError_t kbk_loo_finalize(const CvParams& p, cudaStream_t st) {
     loo_finalize_kernel<<<(p.n + 127) / 128, 128, 0, st>>>(p);
     return cudaGetLastError();
 }
 
-cudaError_t kbk_loo_pairs(int dim, int n, const double* ax, const double* ay, const double* az, double eps, int* cnt,
-                          const int* off, int* pj, double* pd, cudaStream_t st) {
+cudaError_t kbk_loo_pairs(int dim, int n, const double* ax, const double* ay, const double* az, double eps,
+                          const int* grp, int* cnt, const int* off, int* pj, double* pd, cudaStream_t st) {
     return KbDims::dispatch(dim, [&](auto D) {
-        loo_pairs_kernel<D><<<(n + 255) / 256, 256, 0, st>>>(n, ax, ay, az, eps, cnt, off, pj, pd);
-        return cudaGetLastError();
+        return KbBools::dispatch(grp != nullptr, [&](auto GRP) {
+            loo_pairs_kernel<D, bool(GRP)><<<(n + 255) / 256, 256, 0, st>>>(n, ax, ay, az, eps, grp, cnt, off, pj, pd);
+            return cudaGetLastError();
+        });
     });
 }
 
-cudaError_t kbk_loo_dup(const LooParams& p, int nst, const int* st_list, const int* off, const int* pj, const double* pd,
+cudaError_t kbk_loo_dup(const CvParams& p, int nst, const int* st_list, const int* off, const int* pj, const double* pd,
                         cudaStream_t st) {
     if (nst == 0) return cudaSuccess;
     loo_dup_kernel<<<(nst + 7) / 8, 256, 0, st>>>(p, nst, st_list, off, pj, pd);
@@ -209,23 +226,17 @@ cudaError_t kbk_loo_dup(const LooParams& p, int nst, const int* st_list, const i
 
 // P_jl = G_jl - u_j^T S^-1 u_l, evaluated in the order (max(j, l), min(j, l)) so that P is exactly symmetric;
 // *usu_out = u_j^T S^-1 u_l
-__device__ double lgo_p(const LgoParams& P, int j, int l, double* usu_out = nullptr) {
+__device__ double lgo_p(const CvParams& P, int j, int l, double* usu_out = nullptr) {
     const int hi = max(j, l), lo = min(j, l);
     const double s = P.G[(size_t)hi * P.ld + lo];
-    const int K1 = P.K1;
-    double usu = 0.0;
-    for (int a = 0; a < K1; ++a) {
-        double t = 0.0;
-        for (int b = 0; b < K1; ++b) t += P.consts[a * K1 + b] * P.Uz[(size_t)b * P.n_pad + lo];
-        usu += P.Uz[(size_t)a * P.n_pad + hi] * t;
-    }
+    const double usu = cv_usu(P, hi, lo);
     if (usu_out) *usu_out = usu;
     return s - usu;
 }
 
 // blk[boff[g] + a m + b] = P_{S_a S_b} for every group g = blockIdx.y (grid-stride over its m^2 entries); the diagonal also
 // gives scale[goff[g] + a] = max(|G_ii|, |u_i^T S^-1 u_i|), the terms whose difference P_ii is
-__global__ void __launch_bounds__(256) lgo_gather_kernel(LgoParams P) {
+__global__ void __launch_bounds__(256) lgo_gather_kernel(CvParams P) {
     const int g = blockIdx.y, o = P.goff[g], m = P.goff[g + 1] - o;
     double* blk = P.blk + P.boff[g];
     for (long long e = (long long)blockIdx.x * 256 + threadIdx.x; e < (long long)m * m; e += (long long)gridDim.x * 256) {
@@ -240,7 +251,7 @@ __global__ void __launch_bounds__(256) lgo_gather_kernel(LgoParams P) {
 // In-place Gauss-Jordan inverse of one small block (m <= LGO_SMALL) in shared memory, one CTA per group: partial
 // pivoting (largest |value|, ties to the lower row), the column swaps in reverse order at the end. A pivot at or below
 // tol * scale of its station means the drift is not determined without the group: *bad = lowest such group.
-__global__ void __launch_bounds__(256) lgo_small_kernel(LgoParams P, const int* __restrict__ glist) {
+__global__ void __launch_bounds__(256) lgo_small_kernel(CvParams P, const int* __restrict__ glist) {
     extern __shared__ __align__(16) double lsm[];
     __shared__ double wv[8]; __shared__ int wi[8];
     __shared__ int fail;
@@ -320,7 +331,7 @@ __global__ void lgo_unpad_kernel(const double* __restrict__ src, int ld, double*
 
 // One thread per station i (group g, position a): e_v = row a of P_SS^-1 . alpha_S,v (b ascending), zhat = Z - e,
 // sigma^2 = (P_SS^-1)_aa. Every product and sum of field v is the same whatever nv is and wherever v sits.
-__global__ void lgo_finalize_kernel(LgoParams P) {
+__global__ void lgo_finalize_kernel(CvParams P) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= P.n) return;
     const int g = P.grp[i], o = P.goff[g], m = P.goff[g + 1] - o, a = P.pos[i];
@@ -336,22 +347,17 @@ __global__ void lgo_finalize_kernel(LgoParams P) {
 }
 
 // Exact-hit correction of station i in S (one warp per station with near stations outside its group), D = D(i) at
-// pj/pd + off[w] (ascending j, at most LOO_MAXDUP), Delta_j = gamma(d_ij), Q = P_SS^-1:
+// pj/pd + off[i] (ascending j, at most LOO_MAXDUP), Delta_j = gamma(d_ij), Q = P_SS^-1:
 //     zhat_v  += sum_j Delta_j (alpha_jv - P_jS e_S,v)
 //     sigma^2 += 2 sum_j Delta_j (P_jS Q)_a - sum_{j,l} Delta_j Delta_l (P_jl - P_jS Q P_Sl)
 // scratch + soff[w]: P_jS (|D| x m), then P_jS Q (|D| x m). Lanes split b; sums over b close with a fixed xor tree.
-__device__ __forceinline__ double lgo_warp_sum(double s) {
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    return s;
-}
-
-__global__ void __launch_bounds__(256) lgo_dup_kernel(LgoParams P, int nst, const int* __restrict__ st,
+__global__ void __launch_bounds__(256) lgo_dup_kernel(CvParams P, int nst, const int* __restrict__ st,
                                                       const int* __restrict__ off, const int* __restrict__ pj,
                                                       const double* __restrict__ pd, const long long* __restrict__ soff,
                                                       double* __restrict__ scratch) {
     const int w = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (w >= nst) return;
-    const int i = st[w], d0 = off[w], cnt = off[w + 1] - d0;
+    const int i = st[w], d0 = off[i], cnt = off[i + 1] - d0;
     const int g = P.grp[i], o = P.goff[g], m = P.goff[g + 1] - o, a = P.pos[i];
     const double* Q = P.blk + P.boff[g];
     double* ps = scratch + soff[w];                  // [cnt][m] P_jS
@@ -375,7 +381,7 @@ __global__ void __launch_bounds__(256) lgo_dup_kernel(LgoParams P, int nst, cons
         for (int u = 0; u < cnt; ++u) {
             double s = 0.0;
             for (int b = lane; b < m; b += 32) s += qs[(size_t)t * m + b] * ps[(size_t)u * m + b];
-            s = lgo_warp_sum(s);
+            s = cv_warp_sum(s);
             quad += dl[t] * dl[u] * (lgo_p(P, pj[d0 + t], pj[d0 + u]) - s);
         }
     }
@@ -386,7 +392,7 @@ __global__ void __launch_bounds__(256) lgo_dup_kernel(LgoParams P, int nst, cons
         for (int t = 0; t < cnt; ++t) {
             double s = 0.0;
             for (int b = lane; b < m; b += 32) s += ps[(size_t)t * m + b] * e[P.mem[o + b]];
-            s = lgo_warp_sum(s);
+            s = cv_warp_sum(s);
             acc += dl[t] * (P.alpha[(size_t)v * P.n + pj[d0 + t]] - s);
         }
         dz[v] = acc;
@@ -397,7 +403,7 @@ __global__ void __launch_bounds__(256) lgo_dup_kernel(LgoParams P, int nst, cons
     }
 }
 
-cudaError_t kbk_lgo_gather(const LgoParams& p, int n_groups, int max_m, cudaStream_t st) {
+cudaError_t kbk_lgo_gather(const CvParams& p, int n_groups, int max_m, cudaStream_t st) {
     const long long e = (long long)max_m * max_m;
     const int bx = (int)std::min<long long>(64, (e + 255) / 256);
     lgo_gather_kernel<<<dim3(bx, n_groups), 256, 0, st>>>(p);
@@ -406,7 +412,7 @@ cudaError_t kbk_lgo_gather(const LgoParams& p, int n_groups, int max_m, cudaStre
 
 size_t kbk_lgo_small_smem(int m) { return (size_t)m * m * sizeof(double) + (size_t)m * (sizeof(double) + 2 * sizeof(int)); }
 
-cudaError_t kbk_lgo_small(const LgoParams& p, int count, const int* glist, int max_m, cudaStream_t st) {
+cudaError_t kbk_lgo_small(const CvParams& p, int count, const int* glist, int max_m, cudaStream_t st) {
     if (count == 0) return cudaSuccess;
     const size_t smem = kbk_lgo_small_smem(max_m);
     KB_CUDA_OK(cudaFuncSetAttribute(lgo_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -424,12 +430,12 @@ cudaError_t kbk_lgo_unpad(const double* src, int ld, double* blk, int m, cudaStr
     return cudaGetLastError();
 }
 
-cudaError_t kbk_lgo_finalize(const LgoParams& p, cudaStream_t st) {
+cudaError_t kbk_lgo_finalize(const CvParams& p, cudaStream_t st) {
     lgo_finalize_kernel<<<(p.n + 127) / 128, 128, 0, st>>>(p);
     return cudaGetLastError();
 }
 
-cudaError_t kbk_lgo_dup(const LgoParams& p, int nst, const int* st_list, const int* off, const int* pj, const double* pd,
+cudaError_t kbk_lgo_dup(const CvParams& p, int nst, const int* st_list, const int* off, const int* pj, const double* pd,
                         const long long* soff, double* scratch, cudaStream_t st) {
     if (nst == 0) return cudaSuccess;
     lgo_dup_kernel<<<(nst + 7) / 8, 256, 0, st>>>(p, nst, st_list, off, pj, pd, soff, scratch);

@@ -45,7 +45,7 @@ class OrdinaryKriging3D(Krige3D):
         ``values`` (shape (N,) or (N, V)) as in execute(values=...). ``pseudo_inv=True`` is refused on the global path
         (NotImplementedError) and ignored by the moving window, as in execute().
         """
-        return self._leave_one_out(n_closest_points, values, backend)
+        return self._cross_validate(None, n_closest_points, values, backend)
 
     def leave_group_out(self, groups, n_closest_points=None, values=None, backend="cuda"):
         """Leave-group-out cross-validation: every station kriged from the stations outside its group, with this
@@ -60,4 +60,4 @@ class OrdinaryKriging3D(Krige3D):
         the other groups (2 <= k <= N - size of the largest group). ``values`` as in execute(values=...).
         ``pseudo_inv=True`` is refused on the global path (NotImplementedError) and ignored by the moving window.
         """
-        return self._leave_group_out(groups, n_closest_points, values, backend)
+        return self._cross_validate(groups, n_closest_points, values, backend)

@@ -189,7 +189,7 @@ class UniversalKriging(Krige2D):
         execute(values=...). Raises ``numpy.linalg.LinAlgError`` naming the station when leaving it out leaves the
         drift terms undetermined, and NotImplementedError with ``pseudo_inv=True``.
         """
-        return self._leave_one_out(None, values, backend)
+        return self._cross_validate(None, None, values, backend)
 
     def leave_group_out(self, groups, values=None, backend="cuda"):
         """Leave-group-out cross-validation: every station kriged from the stations outside its group, with this
@@ -203,4 +203,4 @@ class UniversalKriging(Krige2D):
         ``values`` as in execute(values=...). Raises ``numpy.linalg.LinAlgError`` naming the group when leaving it
         out leaves the drift terms undetermined, and NotImplementedError with ``pseudo_inv=True``.
         """
-        return self._leave_group_out(groups, None, values, backend)
+        return self._cross_validate(groups, None, values, backend)

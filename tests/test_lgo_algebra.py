@@ -12,7 +12,7 @@ import pytest
 import scipy.linalg
 
 import cases
-from lgo_emulator import LgoEmulatedHandle, brute_force_lgo, near_pairs
+from cv_emulator import CvEmulatedHandle as LgoEmulatedHandle, brute_force_lgo, near_pairs
 from oracle import krige_oracle as ko
 from test_loo_algebra import _c0, _rescale
 

@@ -14,7 +14,7 @@ import scipy.linalg
 from scipy.spatial.distance import cdist
 
 import cases
-from lgo_emulator import brute_force_lgo, _refined_solve_many
+from cv_emulator import brute_force_lgo, _refined_solve_many
 from oracle import krige_oracle as ko
 from test_loo_gpu import EXP, GLOBAL, _build, _obj, _reference_inputs, _stations
 

@@ -12,7 +12,7 @@ import pytest
 from numpy.testing import assert_array_equal
 
 import cases
-from lgo_emulator import LgoEmulatedHandle
+from cv_emulator import CvEmulatedHandle as LgoEmulatedHandle
 
 EXP = [1.0, 300.0, 0.05]
 KINDS = ["ok", "uk", "ok3d", "uk3d"]

@@ -15,7 +15,7 @@ import scipy.linalg
 from scipy.spatial.distance import cdist
 
 import cases
-from loo_emulator import LooEmulatedHandle, brute_force_loo
+from cv_emulator import CvEmulatedHandle as LooEmulatedHandle, brute_force_loo
 from oracle import krige_oracle as ko
 
 TOL = 1e-9          # max|covariance form - brute force| / max|brute force|, z and sigma^2

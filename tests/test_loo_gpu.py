@@ -11,7 +11,7 @@ import numpy as np
 import pytest
 
 import cases
-from loo_emulator import _refined_solve, brute_force_loo
+from cv_emulator import _refined_solve, brute_force_loo
 from oracle import krige_oracle as ko
 
 pytestmark = pytest.mark.gpu

@@ -11,7 +11,7 @@ import pytest
 from numpy.testing import assert_array_equal
 
 import cases
-from loo_emulator import LooEmulatedHandle
+from cv_emulator import CvEmulatedHandle as LooEmulatedHandle
 
 EXP = [1.0, 300.0, 0.05]
 
