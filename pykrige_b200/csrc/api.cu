@@ -15,8 +15,9 @@
 
 #define KB_VERSION 2000
 static const int64_t KB_STAGE_PTS = 1 << 20;   // prediction points per staged output chunk (2 x 8 MB through pinned memory)
-#define KB_TILE_COST_32 0.607     // one round of 32-point tiles relative to one round of 64-point tiles (fp64 kernel, N=5000,
-#define KB_TILE_COST_16 0.403     // one H100 80GB HBM3 at 400 W: 5.26 / 3.19 / 2.12 ms per round; scripts/tile_timing.py)
+#define KB_TILE_COST_32 0.534     // one round of 32-point tiles relative to one round of 64-point tiles (fp64 kernel, N=5000,
+#define KB_TILE_COST_16 0.432     // one H100 80GB HBM3 at 700 W: 3.90 / 2.08 / 1.68 ms per round at an uncapped
+                                  // 1965-1980 MHz SM clock; scripts/tile_timing.py)
 static const int64_t KB_STAGE_MIN = 1 << 18;   // below this the outputs go straight to the caller's buffers
 #define KB_TN_FIELDS 32   // widest point tile of the value-fields solve kernels (solve.cu: no spills up to 32 points)
 

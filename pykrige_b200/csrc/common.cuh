@@ -213,21 +213,32 @@ __device__ __forceinline__ void kb_dmma(double& c0, double& c1, double a, double
                  : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
 }
 
-// ---- mma.sync m16n8k4 f64 (SASS DMMA.16x8x4): the shape of the fp64 solve kernel --------------------------------
-// g = lane >> 2, t = lane & 3.  A 16x4 row: a[i] = A[g + 8 i][t];  B 4x8 col: b = B[t][g];  C 16x8: c[i] = C[g + 8 (i >> 1)][2t + (i & 1)]
-// (tests/test_dmma_fragments_gpu.py pins these maps). On H100 the 16x8xK shapes run at twice the per-FMA rate of
-// m8n8k4 (scripts/dmma_rate.py); k = 4 keeps the operand registers per MMA smallest.
-__device__ __forceinline__ void kb_dmma_16x8x4(double* c, const double* a, double b) {
-    asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+// ---- mma.sync m16n8k16 f64 (SASS DMMA.16x8x16): the shape of the fp64 solve kernel --------------------------------
+// g = lane >> 2, t = lane & 3.  A 16x16 row: a[i] = A[g + 8 (i & 1)][t + 4 (i >> 1)];  B 16x8 col: b[i] = B[t + 4 i][g];
+// C 16x8: c[i] = C[g + 8 (i >> 1)][2t + (i & 1)]  (tests/test_dmma_fragments_gpu.py pins these maps). On H100 the
+// 16x8xK shapes run at twice the per-FMA rate of m8n8k4 (scripts/dmma_rate.py); k = 16 reads and writes the 16x8
+// accumulator once per 2048 FMA instead of once per 512 (k = 4), and takes one issue slot per 2048 FMA.
+__device__ __forceinline__ void kb_dmma_16x8x16(double* c, const double* a, const double* b) {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
+                 "{%12,%13,%14,%15}, {%0,%1,%2,%3};\n"
                  : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
-                 : "d"(a[0]), "d"(a[1]), "d"(b));
+                 : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]),
+                   "d"(b[0]), "d"(b[1]), "d"(b[2]), "d"(b[3]));
 }
 
 // W tile order of the fp64 solve kernel (KB_BM x KB_BK, element (r, k)):  [m16 tile r/16][k/4][lane (r%8)*4 + k%4][(r/8)%2]
-// = the m16n8k4 A fragment (rows g and g + 8) of each lane as one double2, so one LDS.128 over the 32 lanes reads 512
-// contiguous bytes (conflict-free); written by pack_kernel / pack_gform_kernel (factor.cu). The RHS tile keeps
-// the m8n8k4-era order ((k/4)*NT + n/8)*32 + (n%8)*4 + k%4, which already is the m16n8k4 B fragment: one LDS.64 over
-// 256 contiguous bytes.
+// (written by pack_kernel / pack_gform_kernel, factor.cu): the double2 at [m16 tile][k4][lane] is a[2 k4], a[2 k4 + 1]
+// of the m16n8k16 A fragment, so a lane's 8 values are 4 LDS.128, each over 512 contiguous bytes of the warp
+// (conflict-free; 64 contiguous bytes per lane would make every LDS.128 a 4-way bank conflict). The RHS tile order
+// ((k/4)*NT + n/8)*32 + (n%8)*4 + k%4 holds b[k4] of n-tile n/8 at [k4][n/8][lane]: 4 LDS.64, each over 256
+// contiguous bytes.
+
+// Per-warpgroup register limit (sm_90a): every warp of a warpgroup executes the same one; .inc waits until the CTA's
+// pool has the registers, .dec returns them.
+template <int R>
+__device__ __forceinline__ void kb_setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" :: "n"(R)); }
+template <int R>
+__device__ __forceinline__ void kb_setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" :: "n"(R)); }
 
 // ---- mbarrier + 1-D bulk copy (TMA engine, SASS UBLKCP): the toolkit of the pipelined kernels ----------------
 __device__ __forceinline__ uint32_t kb_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }

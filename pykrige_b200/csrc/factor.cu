@@ -612,7 +612,7 @@ __global__ void __launch_bounds__(256) dual_small_kernel(int n, int n_pad, int K
 
 // ---------------------------------------------------------------------------
 // K2d  pack: tile (row block I, k tile kt) -> 4096 values in the fp64 solve kernel's order: element (r, k) of the tile
-//   lives at ((r/16)*4 + k/4)*64 + ((r%8)*4 + k%4)*2 + (r/8)%2, the m16n8k4 A-fragment order of common.cuh.
+//   lives at ((r/16)*4 + k/4)*64 + ((r%8)*4 + k%4)*2 + (r/8)%2, the m16n8k16 A-fragment order of common.cuh.
 // rows < n: W (lower triangle); rows [n, n+na): dual rows Uz^T; other rows 0.
 __device__ __forceinline__ void pack_rk(int I, int kt, int e, int& r, int& k) {
     // e = ((m16 tile * 4 + k/4) * 32 + lane) * 2 + (r/8)%2, lane = (r%8)*4 + k%4

@@ -8,7 +8,7 @@
 //     g_j  = U^T c_j, zc_j = zeta . c_j   <- extra dense "dual rows" appended to W (same GEMM)
 //     finalize: r = g - f_j, mu = S^-1 r, sigma2 = c0 - q + r.mu, z = zc - mu.phi
 //
-// Kernels in this file (all fp64, mma.sync.m16n8k4 = SASS DMMA.16x8x4; on H100 the 16x8xK shapes run at twice the
+// Kernels in this file (all fp64, mma.sync.m16n8k16 = SASS DMMA.16x8x16; on H100 the 16x8xK shapes run at twice the
 // per-FMA rate of m8n8k4, 127 vs 64 FMA/clk/SM, scripts/dmma_rate.py):
 //   solve_kernel_pt   (K3 v3, the product path) persistent CTAs, one CTA = 64 points x all rows of W, RHS column
 //                     block generated once per tile, W/RHS tiles streamed by cp.async.bulk + mbarrier, fused
@@ -24,21 +24,24 @@
 // recompute of sqrt+exp at N=5000 - and alternates generation with the tensor work (measured: DMMA pipe
 // 54 % active). v2 (warp-specialised but still regenerating) was slower: four producer warps cannot
 // hide the fp64 sqrt/exp latency. v3 removes the recompute instead:
-//   phase G  all 12 warps evaluate the RHS column block c[k][j] of the tile ONCE (n x 64 values) and
+//   phase G  the 8 consumer warps evaluate the RHS column block c[k][j] of the tile ONCE (n x 64 values) and
 //            park it, already in MMA-fragment order, in a per-CTA scratch ring (L2-resident, re-used for
 //            every tile the CTA processes; size independent of M);
 //   phase M  warp 0 streams W tiles (32 KB) and RHS tiles (8 KB) with cp.async.bulk + mbarrier into a
-//            5-stage ring; warps 4..11 do nothing but LDS + m16n8k4 DMMA, walking all row blocks; each owns
+//            5-stage ring; warps 4..11 do nothing but LDS + m16n8k16 DMMA, walking all row blocks; each owns
 //            the 16-row m-tiles j and 15 - j of a block (2 x NT x 4 accumulators) and adds its per-point sums
-//            of squares to shared memory at the end of every row block (registers go to the accumulators:
-//            a CTA of 12 warps gets 168 per thread, and fewer warps would not raise that, as three warps
-//            still share one SM sub-partition's 64 KB register file);
+//            of squares to shared memory at the end of every row block (a CTA of 12 warps gets 168 registers
+//            per thread; warps 0..3 need few and hand theirs to the consumers with setmaxnreg: 56 / 224);
 //   phase F  the (K+1)x(K+1) drift solve and the two outputs per point are produced in the same CTA:
 //            no partial buffers, no separate finalize pass, fixed summation order (deterministic).
 #define PT_STAGES 5
 #define PT_THREADS 384
 #define PT_CONS0 (PT_THREADS / 32 - 8)    // first of the 8 consumer warps
 #define PT_STAGE_BYTES ((KB_BM * KB_BK + KB_BK * KB_TN) * 8)
+// registers per thread of warpgroup 0 and of the consumer warpgroups (setmaxnreg) and at launch (__launch_bounds__):
+// 128 x 56 + 256 x 224 = 384 x 168
+#define PT_REGS_PRODUCER 56
+#define PT_REGS_CONSUMER 224
 
 // Sum of v[0..CNT) over the 8 lanes of a warp that share lane & 3 (the row lanes of an MMA C fragment), halving the
 // values at each of the butterfly steps xor 16, 8, 4: afterwards v[0..max(CNT/8, 1)) hold this lane's share of the sums.
@@ -75,6 +78,43 @@ __device__ __forceinline__ int pt_reduce_scatter_index(int i, int lane) {
     return o;
 }
 
+// Phase M of one consumer warp over the stages [g, gto) of the ring: wait for each, run one m16n8k16 per (m-tile,
+// n-tile) for the m-tiles in ON (bit q: m-tile mt[q]), release the stage. ON is a template argument, so no mma.sync sits
+// behind a branch the compiler cannot prove warp-uniform (that costs a WARPSYNC before every DMMA).
+template <int NT, int ON>
+__device__ __forceinline__ void pt_stages(uint32_t& g, uint32_t gto, double (&acc)[2][NT][4], const double* Ts,
+                                          const double* Bs, uint64_t* full, uint64_t* empty, const int (&mt)[2], int lane) {
+    for (; g < gto; ++g) {
+        const int s = g % PT_STAGES;
+        // every consumer waits for every stage (also the ones it skips) so that no warp can lap the ring and arrive
+        // twice on empty[s] within one phase
+        kb_mbar_wait(&full[s], (uint32_t)((g / PT_STAGES) & 1));
+        if constexpr (ON != 0) {
+            const double2* ts = reinterpret_cast<const double2*>(Ts + (size_t)s * KB_BM * KB_BK);
+            const double* bs = Bs + (size_t)s * KB_BK * NT * 8;
+            double fa[2][8];
+#pragma unroll
+            for (int q = 0; q < 2; ++q)
+                if (ON >> q & 1)
+#pragma unroll
+                    for (int k4 = 0; k4 < 4; ++k4) {
+                        const double2 v = ts[(mt[q] * 4 + k4) * 32 + lane];
+                        fa[q][2 * k4] = v.x; fa[q][2 * k4 + 1] = v.y;
+                    }
+#pragma unroll
+            for (int nt = 0; nt < NT; ++nt) {
+                double fb[4];
+#pragma unroll
+                for (int k4 = 0; k4 < 4; ++k4) fb[k4] = bs[(k4 * NT + nt) * 32 + lane];
+                if (ON & 1) kb_dmma_16x8x16(acc[0][nt], fa[0], fb);
+                if (ON & 2) kb_dmma_16x8x16(acc[1][nt], fa[1], fb);
+            }
+        }
+        __syncwarp();
+        if (lane == 0) kb_mbar_arrive(&empty[s]);
+    }
+}
+
 // NT = n-tiles (of 8 points) per point tile: 8 (64 points) is the default. Narrower tiles (NT = 4, 2: 32 / 16 points) are used by
 // the host for the TAIL of a launch: the points left over after the last full round of 64-point tiles would keep only a few of
 // the persistent CTAs (one per SM) busy for a whole tile time (1953 tiles on 132 SMs = 14.8 rounds at 125 000 points per
@@ -108,50 +148,56 @@ __global__ void __launch_bounds__(PT_THREADS, 1) solve_kernel_pt(const __grid_co
     // stages of one tile (W tiles of all row blocks); the running stage counter of a tile starts at (tiles this CTA
     // already did) x this, the same sequence in producer and consumers (recomputed per tile: no register held)
     const uint32_t stages_per_tile = (uint32_t)(P.pm.tile_off[P.nrb - 1] + P.pm.ktiles[P.nrb - 1]);
-    const int cw = warp - PT_CONS0;   // consumer warp 0..7
+    // consumer warp 0..7, read from lane 0 so that the compiler knows it (and the m-tile limits of phase M computed
+    // from it) to be warp-uniform
+    const int cw = __shfl_sync(0xffffffffu, warp - PT_CONS0, 0);
 
-    // the loop counts this CTA's tiles in 32 bits and forms the 64-bit tile index where it is used: registers are
-    // scarce in phase M (the accumulators take 128 of the 168)
-    for (uint32_t it = 0; blockIdx.x + (long long)it * gridDim.x < ntiles; ++it) {
-        const long long tile = blockIdx.x + (long long)it * gridDim.x;
-        const uint32_t git = it * stages_per_tile;
-        // ---------------- phase G: RHS column block of this tile, once ----------------
-        {
-            const int pl = tid % TN;                 // point within the tile
-            const int ks = tid / TN;                 // k-tile slice (6 slices at 64 points, 8 at 48)
-            const long long pj = tile * TN + pl;
-            const bool pvalid = pj < P.m;
-            double px = 0.0, py = 0.0, pz = 0.0;
-            if (pvalid) kb_load_point<DIM>(P.ps, P.an, pj, px, py, pz);
-            for (int t = ks; t < nk; t += PT_THREADS / TN) {
-                double* bt = scratch + (size_t)t * (KB_BK * TN);
+    // ---------------- phase G: RHS column block of a tile, once, by the 8 consumer warps ----------------
+    auto phase_g = [&](long long tile) {
+        const int ct = tid - PT_CONS0 * 32;
+        const int pl = ct % TN;                  // point within the tile
+        const int ks = ct / TN;                  // k-tile slice (4 slices at 64 points)
+        const long long pj = tile * TN + pl;
+        const bool pvalid = pj < P.m;
+        double px = 0.0, py = 0.0, pz = 0.0;
+        if (pvalid) kb_load_point<DIM>(P.ps, P.an, pj, px, py, pz);
+        for (int t = ks; t < nk; t += (PT_THREADS - PT_CONS0 * 32) / TN) {
+            double* bt = scratch + (size_t)t * (KB_BK * TN);
 #pragma unroll
-                for (int k4 = 0; k4 < 4; ++k4) {
-                    double v[4];
+            for (int k4 = 0; k4 < 4; ++k4) {
+                double v[4];
 #pragma unroll
-                    for (int kk = 0; kk < 4; ++kk) {
-                        const int k = t * KB_BK + k4 * 4 + kk;
-                        double val = 0.0;
-                        if (pvalid && k < P.n) {
-                            double d = kb_dist<DIM>(__ldg(P.ax + k), __ldg(P.ay + k), KB_HASZ(DIM) ? __ldg(P.az + k) : 0.0,
-                                                    px, py, pz);
-                            val = kb_cov_rhs<MODEL>(P.vg, d);
-                        }
-                        v[kk] = val;
+                for (int kk = 0; kk < 4; ++kk) {
+                    const int k = t * KB_BK + k4 * 4 + kk;
+                    double val = 0.0;
+                    if (pvalid && k < P.n) {
+                        double d = kb_dist<DIM>(__ldg(P.ax + k), __ldg(P.ay + k), KB_HASZ(DIM) ? __ldg(P.az + k) : 0.0,
+                                                px, py, pz);
+                        val = kb_cov_rhs<MODEL>(P.vg, d);
                     }
-                    // fragment order ((k4*NT + n/8)*32 + (n%8)*4 + k%4): 4 consecutive k = 32 contiguous bytes
-                    double2* dst = reinterpret_cast<double2*>(bt + (k4 * NT + (pl >> 3)) * 32 + (pl & 7) * 4);
-                    dst[0] = make_double2(v[0], v[1]);
-                    dst[1] = make_double2(v[2], v[3]);
+                    v[kk] = val;
                 }
+                // fragment order ((k4*NT + n/8)*32 + (n%8)*4 + k%4): 4 consecutive k = 32 contiguous bytes
+                double2* dst = reinterpret_cast<double2*>(bt + (k4 * NT + (pl >> 3)) * 32 + (pl & 7) * 4);
+                dst[0] = make_double2(v[0], v[1]);
+                dst[1] = make_double2(v[2], v[3]);
             }
-            kb_fence_publish_async();      // the bulk copies of this CTA read the ring
         }
-        __syncthreads();
+        kb_fence_publish_async();      // the bulk copies of this CTA read the ring
+    };
 
-        // ---------------- phase M ----------------
-        if (warp == 0) {
-            if (lane == 0) {
+    // The warps keep one role for the whole kernel. In warpgroup 0 (warps 0..3) warp 0 streams the ring in phase M and
+    // the others wait; it lends registers to the consumer warpgroups (warps 4..11), which hold the accumulators and the
+    // operand fragments of two m-tiles in phase M and run phases G and F (ptxas 12.9 crashes on phase G's geographic
+    // distance code in warpgroup 0's register-reduced region). Both loops pass the same three barriers per tile. The loops count this CTA's
+    // tiles in 32 bits and form the 64-bit tile index where it is used.
+    if (warp < PT_CONS0) {
+        kb_setmaxnreg_dec<PT_REGS_PRODUCER>();
+        for (uint32_t it = 0; blockIdx.x + (long long)it * gridDim.x < ntiles; ++it) {
+            __syncthreads();      // phase G
+            // ---------------- phase M: the producer ----------------
+            const uint32_t git = it * stages_per_tile;
+            if (warp == 0 && lane == 0) {
                 uint32_t g = git;
                 const uint64_t pol_w = kb_policy_evict_last(), pol_c = kb_policy_evict_first();
                 long long tau = 0;                   // W tiles are stored contiguously in (I, t) order
@@ -168,7 +214,17 @@ __global__ void __launch_bounds__(PT_THREADS, 1) solve_kernel_pt(const __grid_co
                     }
                 }
             }
-        } else if (warp >= PT_CONS0) {
+            __syncthreads();
+            __syncthreads();      // phase F
+        }
+    } else {
+        kb_setmaxnreg_inc<PT_REGS_CONSUMER>();
+        for (uint32_t it = 0; blockIdx.x + (long long)it * gridDim.x < ntiles; ++it) {
+            const long long tile = blockIdx.x + (long long)it * gridDim.x;
+            phase_g(tile);
+            __syncthreads();
+            // ---------------- phase M: the consumers ----------------
+            const uint32_t git = it * stages_per_tile;
             uint32_t g = git;
             // running per-point sums of this warp, kept in its row of qred (registers are spent on the accumulators):
             // after the reduce-scatter of each row-block epilogue, sum v of this lane belongs to (n-tile, column)
@@ -202,34 +258,13 @@ __global__ void __launch_bounds__(PT_THREADS, 1) solve_kernel_pt(const __grid_co
                     for (int b = 0; b < NT; ++b)
 #pragma unroll
                         for (int i = 0; i < 4; ++i) acc[a][b][i] = 0.0;
-                for (; g < gend; ++g) {
-                    const int s = g % PT_STAGES;
-                    // every consumer waits for every stage (also the ones it skips) so that no warp can lap
-                    // the ring and arrive twice on empty[s] within one phase
-                    kb_mbar_wait(&full[s], (uint32_t)((g / PT_STAGES) & 1));
-                    const bool on0 = g < glim[0], on1 = g < glim[1];
-                    if (on0 || on1) {
-                        const double2* ts = reinterpret_cast<const double2*>(Ts + (size_t)s * KB_BM * KB_BK);
-                        const double* bs = Bs + (size_t)s * KB_BK * TN;
-#pragma unroll
-                        for (int k4 = 0; k4 < 4; ++k4) {         // four m16n8k4 steps per k tile, k ascending
-                            double fa[2][2];
-#pragma unroll
-                            for (int q = 0; q < 2; ++q) {
-                                const double2 v = ts[(mtl[q] * 4 + k4) * 32 + lane];
-                                fa[q][0] = v.x; fa[q][1] = v.y;
-                            }
-#pragma unroll
-                            for (int nt = 0; nt < NT; ++nt) {
-                                const double fb = bs[(k4 * NT + nt) * 32 + lane];
-                                if (on0) kb_dmma_16x8x4(acc[0][nt], fa[0], fb);
-                                if (on1) kb_dmma_16x8x4(acc[1][nt], fa[1], fb);
-                            }
-                        }
-                    }
-                    __syncwarp();
-                    if (lane == 0) kb_mbar_arrive(&empty[s]);
-                }
+                // each m-tile's k tiles are a prefix of the block's stages: both m-tiles up to the smaller limit, then
+                // the one with the larger limit alone, then neither (the stages are still waited for and released)
+                const uint32_t glo = min(min(glim[0], glim[1]), gend), ghi = min(max(glim[0], glim[1]), gend);
+                pt_stages<NT, 3>(g, glo, acc, Ts, Bs, full, empty, mtl, lane);
+                if (glim[0] > glim[1]) pt_stages<NT, 1>(g, ghi, acc, Ts, Bs, full, empty, mtl, lane);
+                else pt_stages<NT, 2>(g, ghi, acc, Ts, Bs, full, empty, mtl, lane);
+                pt_stages<NT, 0>(g, gend, acc, Ts, Bs, full, empty, mtl, lane);
                 // row-block epilogue, in place: every accumulator of a W row becomes its term of the point's sum (square,
                 // or c[r] times it for the quadratic form), dual rows go to shared memory and, like padding rows, add 0;
                 // then the warp's per-point sums (fixed order: m-tile, row g before g + 8) are reduced over the 8 row
@@ -287,23 +322,24 @@ __global__ void __launch_bounds__(PT_THREADS, 1) solve_kernel_pt(const __grid_co
                     if (o >= 0) qrow[(o >> 1) * 8 + 2 * (lane & 3) + (o & 1)] += part[v];
                 }
             }
-        }
-        __syncthreads();
+            __syncthreads();
 
-        // ---------------- phase F: per-point finalize (DESIGN.md §3) ----------------
-        if (tid < TN) {
-            const long long pj = tile * TN + tid;
-            if (pj < P.m) {
-                double q = 0.0;
+            // ---------------- phase F: per-point finalize (DESIGN.md §3), one consumer thread per point ----------------
+            const int ft = tid - PT_CONS0 * 32;
+            if (ft < TN) {
+                const long long pj = tile * TN + ft;
+                if (pj < P.m) {
+                    double q = 0.0;
 #pragma unroll
-                for (int w = 0; w < 8; ++w) q += qred[w * TN + tid];     // fixed order: deterministic
-                if constexpr (FIELDS)
-                    kb_finalize_point<DIM, double, true>(P, pj, q, P.fstage + (int)(blockIdx.x * P.na * TN) + tid, TN);
-                else
-                    kb_finalize_point<DIM, double>(P, pj, q, auxs + tid, TN);
+                    for (int w = 0; w < 8; ++w) q += qred[w * TN + ft];     // fixed order: deterministic
+                    if constexpr (FIELDS)
+                        kb_finalize_point<DIM, double, true>(P, pj, q, P.fstage + (int)(blockIdx.x * P.na * TN) + ft, TN);
+                    else
+                        kb_finalize_point<DIM, double>(P, pj, q, auxs + ft, TN);
+                }
             }
+            __syncthreads();      // qred / auxs / scratch are re-used by the next tile
         }
-        __syncthreads();      // qred / auxs / scratch are re-used by the next tile
     }
 }
 

@@ -1,10 +1,12 @@
 // dmma_rate.cu — fp64 tensor-core (DMMA) throughput and fragment-map probe for sm_90a.
 //
 // Built by pykrige_b200/csrc/Makefile into scripts/libdmma_rate.so (not part of libkrige_b200.so); driven by
-// scripts/dmma_rate.py and tests/test_dmma_fragments_gpu.py through two C entry points:
+// scripts/dmma_rate.py and tests/test_dmma_fragments_gpu.py through three C entry points:
 //   dmma_rate_run   steady-state rate of one mma.sync shape: one CTA per SM, 4 * warps_per_smsp warps, every warp
 //                   issues DR_ACC independent MMAs per iteration (enough to cover the DMMA latency), per-CTA clock64
 //                   cycles and the launch time by CUDA events;
+//   dmma_stage_run  one phase-M stage of the fp64 solve kernel repeated for as long as asked (operands from shared
+//                   memory, m16n8k4 or m16n8k16): scripts/dmma_rate.py --sustain samples power and clock around it;
 //   dmma_frag_run   one MMA of one shape on one warp, D = A B + C with row-major A (M x K), B (K x 8), C / D (M x 8):
 //                   the per-lane fragment maps below are exactly what the solve kernel assumes.
 // Shapes: 0 = m8n8k4, 1 = m16n8k4, 2 = m16n8k8, 3 = m16n8k16 (all .row.col.f64).
@@ -105,6 +107,63 @@ __global__ void frag_kernel(const double* __restrict__ A, const double* __restri
     }
 }
 
+// One 16-deep stage of the fp64 solve kernel's phase M, repeated: 8 warps per CTA (2 per SM sub-partition, as the
+// consumer warpgroups), each multiplying the A fragments of two 16-row m-tiles by the B fragments of 8 n-tiles, all read
+// from shared memory in the solve kernel's tile orders. K = 4: four m16n8k4 per (m-tile, n-tile) per stage, K = 16: one
+// m16n8k16. The stage index cycles over ST_STAGES buffers so that the loads cannot be hoisted out of the loop.
+#define ST_STAGES 4
+template <int K>
+__global__ void __launch_bounds__(256, 1) stage_kernel(long long iters, double* __restrict__ out) {
+    __shared__ double2 ta[ST_STAGES][2 * 4 * 32];      // [stage][m-tile][k4][lane]: a[2 k4], a[2 k4 + 1]
+    __shared__ double tb[ST_STAGES][4 * 8 * 32];       // [stage][k4][n-tile][lane]: b[k4]
+    const int lane = threadIdx.x & 31;
+    for (int i = threadIdx.x; i < ST_STAGES * 2 * 4 * 32; i += blockDim.x)
+        (&ta[0][0])[i] = make_double2(1e-3 * ((i % 7) + 1), 1e-3 * ((i % 5) + 1));
+    for (int i = threadIdx.x; i < ST_STAGES * 4 * 8 * 32; i += blockDim.x) (&tb[0][0])[i] = 1e-3 * ((i % 3) + 1);
+    __syncthreads();
+    double acc[2][8][4];
+#pragma unroll
+    for (int q = 0; q < 2; ++q)
+#pragma unroll
+        for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) acc[q][nt][i] = 0.0;
+    for (long long it = 0; it < iters; ++it) {
+        const int s = (int)(it % ST_STAGES);
+        double fa[2][8];
+#pragma unroll
+        for (int q = 0; q < 2; ++q)
+#pragma unroll
+            for (int k4 = 0; k4 < 4; ++k4) {
+                const double2 v = ta[s][(q * 4 + k4) * 32 + lane];
+                fa[q][2 * k4] = v.x; fa[q][2 * k4 + 1] = v.y;
+            }
+#pragma unroll
+        for (int nt = 0; nt < 8; ++nt) {
+            double fb[4];
+#pragma unroll
+            for (int k4 = 0; k4 < 4; ++k4) fb[k4] = tb[s][(k4 * 8 + nt) * 32 + lane];
+#pragma unroll
+            for (int q = 0; q < 2; ++q) {
+                if (K == 16) {
+                    mma<3>(acc[q][nt], fa[q], fb);
+                } else {
+#pragma unroll
+                    for (int k4 = 0; k4 < 4; ++k4) mma<1>(acc[q][nt], &fa[q][2 * k4], &fb[k4]);
+                }
+            }
+        }
+    }
+    double r = 0.0;
+#pragma unroll
+    for (int q = 0; q < 2; ++q)
+#pragma unroll
+        for (int nt = 0; nt < 8; ++nt)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) r += acc[q][nt][i];
+    out[blockIdx.x * blockDim.x + threadIdx.x] = r;
+}
+
 static const int kM[4] = {8, 16, 16, 16};
 static const int kK[4] = {4, 4, 8, 16};
 
@@ -158,6 +217,35 @@ done:
     cudaFree(in);
     cudaFree(out);
     cudaFree(cyc);
+    return (int)e;
+}
+
+// Runs stage_kernel<k> (k = 4 or 16) once on every SM for `iters` stages per warp. Returns cudaError_t; *ms = launch
+// time (CUDA events), *fmas = FMAs of the whole launch. Blocks until the kernel ends (ctypes releases the GIL, so a
+// Python thread can sample NVML meanwhile).
+int dmma_stage_run(int k, long long iters, float* ms, long long* fmas) {
+    if ((k != 4 && k != 16) || iters < 1) return (int)cudaErrorInvalidValue;
+    int dev = 0, nsm = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
+    if (e != cudaSuccess) return (int)e;
+    double* out = nullptr;
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    if ((e = cudaMalloc(&out, sizeof(double) * nsm * 256)) != cudaSuccess) goto done;
+    if ((e = cudaEventCreate(&e0)) != cudaSuccess) goto done;
+    if ((e = cudaEventCreate(&e1)) != cudaSuccess) goto done;
+    cudaEventRecord(e0);
+    if (k == 16) stage_kernel<16><<<nsm, 256>>>(iters, out);
+    else stage_kernel<4><<<nsm, 256>>>(iters, out);
+    cudaEventRecord(e1);
+    if ((e = cudaGetLastError()) != cudaSuccess) goto done;
+    if ((e = cudaEventSynchronize(e1)) != cudaSuccess) goto done;
+    cudaEventElapsedTime(ms, e0, e1);
+    *fmas = iters * (long long)nsm * 8 * (2 * 8 * 16 * 8 * 16);     // warps x (2 m-tiles x 8 n-tiles x 16x8x16)
+done:
+    if (e0) cudaEventDestroy(e0);
+    if (e1) cudaEventDestroy(e1);
+    cudaFree(out);
     return (int)e;
 }
 
