@@ -13,13 +13,16 @@ from .ok3d import OrdinaryKriging3D
 from .uk3d import UniversalKriging3D
 
 try:
-    from sklearn.base import BaseEstimator, RegressorMixin
+    from sklearn.base import BaseEstimator, ClassifierMixin, RegressorMixin
 
     SKLEARN_INSTALLED = True
 except ImportError:  # pragma: no cover
     SKLEARN_INSTALLED = False
 
     class RegressorMixin:  # minimal stand-ins so the class can be defined
+        pass
+
+    class ClassifierMixin:
         pass
 
     class BaseEstimator:
@@ -46,9 +49,27 @@ krige_methods_kws = {
 }
 
 
+class SklearnException(Exception):
+    """scikit-learn is needed but not installed."""
+
+
 def validate_method(method):
     if method not in krige_methods:
         raise ValueError("Kriging method must be one of {}".format(krige_methods.keys()))
+
+
+def validate_sklearn():
+    """Raises SklearnException without scikit-learn (compat.py:89-94): rk.py and ck.py call it on import."""
+    if not SKLEARN_INSTALLED:
+        raise SklearnException("sklearn needs to be installed in order to use this module")
+
+
+def check_sklearn_model(model, task="regression"):
+    """RuntimeError unless `model` is a scikit-learn estimator of the given task, 'regression' or 'classification'
+    (compat.py:294-307)."""
+    mixin = {"regression": RegressorMixin, "classification": ClassifierMixin}.get(task)
+    if mixin is not None and not (isinstance(model, BaseEstimator) and isinstance(model, mixin)):
+        raise RuntimeError("Needs to supply an instance of a scikit-learn %s class." % task)
 
 
 class Krige(RegressorMixin, BaseEstimator):
