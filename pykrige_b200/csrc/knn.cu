@@ -606,10 +606,13 @@ __device__ __forceinline__ void knn_solve_body(const KnnParams& P, int warps_per
             }
             __syncwarp();
         }
-        const double inv = 1.0 / A[pcol * S + pcol];
+        // the multiplier is a true quotient, not a product with the reciprocal: a row equal to the pivot row (coincident
+        // stations, nugget 0) then gets l = 1 exactly and cancels to an exact zero row, so the system is found singular
+        // (a reciprocal can leave l one ulp off 1 and the contracted update a +-ulp row that passes as a pivot)
+        const double piv = A[pcol * S + pcol];
         const double bc = rc[pcol], b1 = r1[pcol];
         for (int i = pcol + 1 + lane; i < k; i += 32) {
-            double l = A[i * S + pcol] * inv;
+            double l = A[i * S + pcol] / piv;
             A[i * S + pcol] = l;
             rc[i] -= l * bc;
             r1[i] -= l * b1;

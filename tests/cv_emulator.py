@@ -21,6 +21,17 @@ from fields_emulator import FieldsEmulatedHandle
 MAXDUP = 32             # LOO_MAXDUP
 
 
+def refined_solution(a, B, steps=2):
+    """x = a^-1 B by oracle.krige_oracle.exec_vector_refined's scheme: one fp64 LU, then `steps` rounds of refinement
+    with the residual B - a x formed and x held in np.longdouble. Returns (x, B) as np.longdouble arrays."""
+    lu = scipy.linalg.lu_factor(a)
+    A, BL = a.astype(np.longdouble), np.asarray(B).astype(np.longdouble)
+    X = scipy.linalg.lu_solve(lu, B).astype(np.longdouble)
+    for _ in range(steps):
+        X += scipy.linalg.lu_solve(lu, (BL - A @ X).astype(np.float64)).astype(np.longdouble)
+    return X, BL
+
+
 def _refined_solve_many(a, P, Q, values, fn, m, exact, dp, steps=2):
     """oracle.krige_oracle.exec_vector_refined's scheme (fp64 LU, refinement with np.longdouble residuals, z and
     sigma^2 summed in np.longdouble) without its condition number, which costs an SVD per call, for several prediction
@@ -34,11 +45,7 @@ def _refined_solve_many(a, P, Q, values, fn, m, exact, dp, steps=2):
     for c, col in enumerate(dp):
         B[n + c] = col
     B[-1] = 1.0
-    lu = scipy.linalg.lu_factor(a)
-    A, BL = a.astype(np.longdouble), B.astype(np.longdouble)
-    X = scipy.linalg.lu_solve(lu, B).astype(np.longdouble)
-    for _ in range(steps):
-        X += scipy.linalg.lu_solve(lu, (BL - A @ X).astype(np.float64)).astype(np.longdouble)
+    X, BL = refined_solution(a, B, steps)
     z = (X[:n].T @ np.asarray(values, dtype=np.longdouble)).astype(np.float64)
     ss = (-np.sum(X * BL, axis=0)).astype(np.float64)
     return z, ss
