@@ -200,8 +200,8 @@ extern "C" int kb200_create(kb200_handle* out, int device) {
     if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) { delete h; return KB200_ECUDA; }
     h->own_stream = true;
     for (auto& ev : h->ev) if (cudaEventCreate(&ev) != cudaSuccess) { delete h; return KB200_ECUDA; }
-    if (kbk_factor_init() != cudaSuccess || kbk_solve_init() != cudaSuccess || kbk_solve_tf32_init() != cudaSuccess ||
-        kbk_solve_i8_init() != cudaSuccess || kbk_ev_init() != cudaSuccess || kbk_pinv_init() != cudaSuccess) { delete h; return KB200_ECUDA; }
+    if (kbk_factor_init() != cudaSuccess || kbk_solve_init() != cudaSuccess || kbk_solve_wgmma_init() != cudaSuccess ||
+        kbk_ev_init() != cudaSuccess || kbk_pinv_init() != cudaSuccess) { delete h; return KB200_ECUDA; }
     if (cudaDeviceGetAttribute(&h->num_sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || h->num_sms < 1) h->num_sms = 132;
     *out = h;
     return KB200_OK;
@@ -748,12 +748,11 @@ extern "C" int kb200_set_device_drift(kb200_handle h, int n_wells, const double*
 static int launch_solve(kb200_ctx* h, const Src& s, double* d_z, double* d_ss, int tp) {
     cudaStream_t st = h->stream;
     const BlobView b = blob_view(h);
-    const bool i8 = h->slices != 0;
-    const bool f32 = h->dtype == KB200_F32;
+    const bool wg = h->dtype != KB200_F64;
     long long ntiles = (s.count + tp - 1) / tp;
     int grid = (int)std::min<long long>(ntiles, h->num_sms);
-    CU(h, h->wScratch.reserve(i8 ? kbk_solve_i8_scratch_bytes(h->slices, h->n, grid) : f32 ? kbk_solve_tf32_scratch_bytes(h->n, grid)
-                                  : kbk_solve_pt_scratch_doubles(h->n, grid) * sizeof(double)));
+    CU(h, h->wScratch.reserve(wg ? kbk_solve_wgmma_scratch_bytes(h->slices, h->n, grid)
+                                 : kbk_solve_pt_scratch_doubles(h->n, grid) * sizeof(double)));
     SolvePtParams pp{};
     pp.vg = h->vg; pp.an = h->an; pp.ps = s.point_source();
     pp.n = h->n; pp.na = h->na; pp.nrb = h->nrb; pp.n_rl = h->n_rl; pp.n_hd = h->n_hd;
@@ -770,8 +769,7 @@ static int launch_solve(kb200_ctx* h, const Src& s, double* d_z, double* d_ss, i
         pp.fstage = h->wFstage.as<double>();
     }
     pp.rowscale = b.rowscale;
-    if (i8) CU(h, kbk_solve_i8(h->slices, h->dim, pp, grid, st));
-    else if (f32) CU(h, kbk_solve_tf32(h->dim, pp, grid, st));
+    if (wg) CU(h, kbk_solve_wgmma(h->slices, h->dim, pp, grid, st));
     else CU(h, kbk_solve_pt(h->dim, pp, grid, tp, st));
     h->launches += 1; h->solve_launches += 1;
     return KB200_OK;
@@ -784,9 +782,7 @@ static double tile_cost(int tp) { return tp == 64 ? 1.0 : (tp == 32 ? KB_TILE_CO
 // NOTE: the summation order per point does not depend on the tile width or on the number of launches either, so the
 // split below is free to choose them.
 static int run_solve(kb200_ctx* h, const Src& s, double* d_z, double* d_ss) {
-    const bool i8 = h->slices != 0;
-    const bool f32 = h->dtype == KB200_F32;
-    if (i8 || f32) return launch_solve(h, s, d_z, d_ss, i8 ? kbk_solve_i8_tile_points() : kbk_solve_tf32_tile_points());
+    if (h->dtype != KB200_F64) return launch_solve(h, s, d_z, d_ss, KB_WG_TM);
     // fp64 DMMA kernel: full rounds of 64-point tiles over all SMs, then the leftover points as ONE more launch whose tile
     // width minimises rounds x cost: a partial round of 64-point tiles keeps a few SMs busy for a whole tile time
     const long long S = h->num_sms;

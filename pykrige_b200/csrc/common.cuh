@@ -301,24 +301,4 @@ __device__ __forceinline__ void kb_bulk_g2s_hint(void* dst, const void* src, uin
                  :: "r"(kb_smem_u32(dst)), "l"(src), "r"(bytes), "r"(kb_smem_u32(bar)), "l"(policy) : "memory");
 }
 
-// ---- warpgroup MMA (wgmma, sm_90a) helpers for the tensor-core solve kernels ---------------------------------
-// Shared-memory matrix descriptor, K-major, no swizzle ("interleave" layout): 8-row x 16-byte core matrices,
-// lbo = byte stride between the two k-adjacent core matrices one instruction reads, sbo = byte stride between
-// 8-row groups. Bits 0-13 start address >> 4, 16-29 lbo >> 4, 32-45 sbo >> 4, layout type (62-63) 0.
-__device__ __forceinline__ uint64_t kb_wgmma_desc(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
-    return (uint64_t)((smem_addr >> 4) & 0x3fffu) | ((uint64_t)((lbo >> 4) & 0x3fffu) << 16) |
-           ((uint64_t)((sbo >> 4) & 0x3fffu) << 32);
-}
-__device__ __forceinline__ void kb_wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
-__device__ __forceinline__ void kb_wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void kb_wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" :: "n"(N) : "memory"); }
-// keeps the compiler from moving accesses of an accumulator register across a wgmma wait
-__device__ __forceinline__ void kb_reg_fence(float& r) { asm volatile("" : "+f"(r) :: "memory"); }
-__device__ __forceinline__ void kb_reg_fence(uint32_t& r) { asm volatile("" : "+r"(r) :: "memory"); }
-// named barrier over the first `threads` threads of the block (id 0 is __syncthreads)
-__device__ __forceinline__ void kb_named_sync(int id, int threads) {
-    asm volatile("bar.sync %0, %1;\n" :: "r"(id), "r"(threads) : "memory");
-}
-
 #define KB_CUDA_OK(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) return _e; } while (0)

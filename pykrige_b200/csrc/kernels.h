@@ -240,27 +240,21 @@ cudaError_t kbk_solve_init();   // opt-in shared memory attributes
 cudaError_t kbk_solve_pt(int dim, const SolvePtParams& p, int grid, int tile_points /* 64 | 32 | 16 */, cudaStream_t st);
 size_t      kbk_solve_pt_scratch_doubles(int n, int grid);
 
-// fp32 path (solve_tf32.cu): wgmma .tf32, 3xTF32 split, fp32 accumulators in registers
-cudaError_t kbk_solve_tf32_init();
-cudaError_t kbk_solve_tf32(int dim, const SolvePtParams& p, int grid, cudaStream_t st);
+// wgmma solve kernels (solve_wgmma.cu): slices = 0 is the float32 path (3xTF32 split, fp32 accumulators), slices =
+// 4 | 5 | 6 the fp64-class path on the INT8 tensor cores (error-free slicing + exact int32 accumulation)
+#define KB_WG_TM 64    // prediction points per CTA tile
+cudaError_t kbk_solve_wgmma_init();
+cudaError_t kbk_solve_wgmma(int slices, int dim, const SolvePtParams& p, int grid, cudaStream_t st);
+size_t      kbk_solve_wgmma_scratch_bytes(int slices, int n, int grid);
 cudaError_t kbk_pack_tf32(const double* W, int ld, int n, int n_pad, int na, const double* Uz, const PackMap& pm,
                           void* out, cudaStream_t st);
-size_t      kbk_solve_tf32_scratch_bytes(int n, int grid);
-int         kbk_solve_tf32_tile_points();
-
-// fp64-class path on the INT8 tensor cores (solve_i8.cu): error-free slicing into S = 4 | 5 | 6 slices + exact int32
-// accumulation
 bool        kbk_i8_valid_slices(int S);
-cudaError_t kbk_solve_i8_init();
-cudaError_t kbk_solve_i8(int S, int dim, const SolvePtParams& p, int grid, cudaStream_t st);
 cudaError_t kbk_pack_i8(int S, const double* W, int ld, int n, int n_pad, int na, const double* Uz,
                         int* rowexp, double* rowscale, const long long* tile_off_dev, void* out, cudaStream_t st);
 int         kbk_i8_nrb(int S, int n, int na);
 int         kbk_i8_rows(int S, int n, int na);
 long long   kbk_i8_total_tiles(int S, int n, int na, long long* tile_off);
 size_t      kbk_i8_tile_bytes(int S);
-size_t      kbk_solve_i8_scratch_bytes(int S, int n, int grid);
-int         kbk_solve_i8_tile_points();
 
 // moving window (knn.cu)
 struct KnnParams {

@@ -13,7 +13,7 @@
 //   solve_kernel_pt   (K3 v3, the product path) persistent CTAs, one CTA = 64 points x all rows of W, RHS column
 //                     block generated once per tile, W/RHS tiles streamed by cp.async.bulk + mbarrier, fused
 //                     finalize. See the comment above the kernel.
-// The wgmma variants live in solve_tf32.cu (dtype float32) and solve_i8.cu (dtype float64x).
+// The wgmma variants (dtype float32 and float64x) live in solve_wgmma.cu.
 #include "common.cuh"
 #include "kernels.h"
 

@@ -1,12 +1,12 @@
-"""fp64-class int8-slice kernels (dtype='float64x' / 'float64x5' / 'float64x4') vs the fp64 DMMA kernel: agreement
-and solve-kernel rate. Prints one JSON line per problem."""
+"""The wgmma kernels (dtype='float64x' / 'float64x5' / 'float64x4' int8 slices, 'float32' 3xTF32) vs the fp64 DMMA
+kernel: agreement and solve-kernel rate. Prints one JSON line per problem."""
 import os, sys, json
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import cases, pykrige_b200 as pk
 
-sizes = ((300, 1000, "ok"), (1000, 20000, "uk"), (5000, 400000, "ok"))
+sizes = ((300, 1000, "ok"), (1000, 20000, "uk"), (5000, 400000, "ok"), (10000, 600000, "uk"))
 if len(sys.argv) > 1 and sys.argv[1] == "big":
     sizes = ((5000, 1000000, "ok"),)
 for n, m, cls in sizes:

@@ -189,12 +189,12 @@ def test_moving_window_model_reproduces_the_reference(t, ref_fuzz):
     np.testing.assert_allclose(ss[keep], sr[keep], rtol=tol, atol=tol * max(np.abs(sr[keep]).max(), 1e-300), err_msg=c["text"])
 
 
-# ---- dtype='float64x' / 'float64x5' / 'float64x4' (csrc/solve_i8.cu): error-free slicing of W rows and RHS columns into
+# ---- dtype='float64x' / 'float64x5' / 'float64x4' (csrc/solve_wgmma.cu): error-free slicing of W rows and RHS columns into
 #      S signed base-128 digits (6 + 7 (S-1) bits), all digit products with d = s + t < S summed exactly in S int32
 #      accumulators, exact int64 recombination, one conversion to fp64 ------------------------------------------------
 def i8_slices(x, e, S):
     """Balanced digits of round(x * 2^(6 + 7 (S-1) - e)): x = 2^e sum_s out[s] 2^(-6-7s) + O(2^(e-7S)), out[s] in [-64, 64]
-    (solve_i8.cu: i8_slice)."""
+    (solve_wgmma.cu: i8_slice)."""
     v = np.rint(np.ldexp(np.asarray(x, dtype=np.float64), 6 + 7 * (S - 1) - e)).astype(np.int64)
     out = np.zeros((S,) + v.shape, dtype=np.int64)
     for s in range(S - 1, 0, -1):
@@ -248,7 +248,7 @@ def test_int8_slice_scheme_is_error_free_and_fp64_class(S, bits, bound):
     assert worst < bound, worst
 
 
-# ---- dtype='float32' (csrc/solve_tf32.cu): 3xTF32 split W = Wh + Wl, c = ch + cl (each part representable in TF32:
+# ---- dtype='float32' (csrc/solve_wgmma.cu): 3xTF32 split W = Wh + Wl, c = ch + cl (each part representable in TF32:
 #      10 explicit mantissa bits, cvt.rna), W c ~= Wh ch + Wh cl + Wl ch accumulated in fp32 ---------------------------
 def tf32_round(x):
     """cvt.rna.tf32.f32: round a float32 to 10 mantissa bits, ties away from zero."""

@@ -1,8 +1,8 @@
 """GPU boundary sweep of the global solve kernels against the extended-precision reference
 (oracle.krige_oracle.exec_vector_refined: the exact solution of the reference's own fp64 gamma-form system).
 
-The fp64 kernel (solve.cu) works on 16-row m-tiles and 16-wide k tiles inside 256-row blocks, the float32 kernel
-(solve_tf32.cu) splits each 256-row block 128/128 over two warpgroups, the float64x kernels (solve_i8.cu) use row
+The fp64 kernel (solve.cu) works on 16-row m-tiles and 16-wide k tiles inside 256-row blocks; of the wgmma kernels
+(solve_wgmma.cu), float32 splits each 256-row block 128/128 over two warpgroups and the float64x ones use row
 blocks of 48 / 64 / 64 rows with k = 32, and the Cholesky panels are 64 and 256 wide. The K + 2 dense dual rows sit
 right after row n. The data sizes below put n and n + na on both sides of each of those boundaries, for ordinary
 kriging (na = 2), universal kriging with a regional-linear drift (na = 4) and with the full 15 drift columns the C ABI
