@@ -390,6 +390,22 @@ int kb200_knn_loo(kb200_handle h, int k, double* z, double* sigmasq);
 int kb200_lgo(kb200_handle h, const int32_t* group, int n_groups, double* z, double* sigmasq);
 int kb200_knn_lgo(kb200_handle h, int k, const int32_t* group, int n_groups, double* z, double* sigmasq);
 
+/* Appended stations (DESIGN.md §5g): the problem kb200_set_problem factored on THIS handle grows by m stations, which
+ * become stations n .. n + m - 1. x, y (z for 3-D), values: m each, in the original coordinates; drift_cols: the n_hd
+ * host drift columns at the new stations (column-major m x n_hd, the order of kb200_set_problem's drift_data), NULL
+ * without drift columns. The held problem keeps its frame (centre, anisotropy, covariance shift c0, drift rescaling):
+ * the new stations are adjusted with the held map. Instead of refactoring, the block row of L and W = L^-1 from the
+ * last full 64-row tile on is extended (L21 = C21 W11^T, L22 = chol(C22 - L21 L21^T), W22 = L22^-1, W21 = -W22 L21 W11,
+ * all on the DMMA pipe), then the dual vectors and the tile stream of the problem's dtype are rebuilt. The execute,
+ * statistics and cross-validation calls then see the n + m stations.
+ * Errors: KB200_EUNSUPPORTED without a global problem factored on this handle, for the pseudo-inverse, the indefinite
+ * fallback or value fields, and for a variogram table whose dmax no longer covers the data (nothing changes);
+ * KB200_EBADARG for m < 1, NULL arrays, or n + m above the limit of kb200_set_problem ("n out of range");
+ * KB200_ESINGULAR when a pivot of the new corner is at or below 16 eps c0, or the drift block becomes singular: the
+ * handle then holds no problem, as after any other error of this call. */
+int kb200_append_data(kb200_handle h, int64_t m, const double* x, const double* y, const double* z,
+                      const double* values, const double* drift_cols);
+
 /* Debug/verification taps (used by tests only): copy device intermediates to host.
  *  what = 1: Cholesky factor L of the shifted covariance matrix (n_pad x n_pad, row-major, lower triangle valid)
  *  what = 2: W = inv(L) (same layout)

@@ -189,6 +189,7 @@ class KrigeBase:
                 [getattr(self, a) for a in self._ANGLES])
 
     def _fit_variogram(self, variogram_parameters, nlags, weight):
+        self._nlags = nlags                     # the experimental variogram of data added later (add_data)
         X, values = self._stats_inputs()
         vp = _make_variogram_parameter_list(self.variogram_model, variogram_parameters)
         self.lags, self.semivariance, self.variogram_model_parameters = _initialize_variogram_model(
@@ -839,6 +840,91 @@ class KrigeBase:
         z, ss = self._per_chunk(fields, run)
         return (z[0] if one else z), ss
 
+    # ---- add_data(): new stations for the held problem ---------------------------------------------------------
+    def _add_data(self, coords, values, specified_drift=None):
+        """The body of add_data() of the four classes. coords = (x, y[, z]) of the new stations in the original frame.
+        Afterwards every public result equals that of an object built with the same arguments, the current variogram
+        as fixed parameters, on the old stations followed by the new ones (DESIGN.md §5g)."""
+        new = [np.atleast_1d(np.squeeze(np.array(a, copy=True, dtype=np.float64))) for a in tuple(coords) + (values,)]
+        m = new[0].size
+        if m == 0 or any(a.ndim != 1 or a.size != m for a in new):
+            raise ValueError("add_data: %s and the values must be 1-D arrays of the same non-zero length, got sizes %s"
+                             % (", ".join(c.lower() for c in self._AXES), [a.size for a in new]))
+        if not all(np.all(np.isfinite(a)) for a in new):
+            raise ValueError("add_data: coordinates and values must be finite")
+        extra = self._new_drift_data(new[:self._ndim], m, specified_drift)
+
+        key = getattr(self, "_kb_key", None)
+        h = getattr(self, "_kb_handle", None)
+        fast = (h is not None and key is not None and not key.knn and key.n_fields == 0 and not key.pseudo_inv
+                and key == self._problem_key(key.dtype, False))
+        frame = self._anisotropy()[0]
+        dmax = getattr(self, "_kb_table_dmax", 0.0)
+
+        names = [c + "_ORIG" for c in self._AXES] + [self._VALUES]
+        for name, a in zip(names, new):
+            setattr(self, name, np.concatenate([getattr(self, name), a]))
+        if self.coordinates_type == "geographic":
+            self.X_ADJUSTED, self.Y_ADJUSTED = self.X_ORIG, self.Y_ORIG
+        else:
+            for c in self._AXES:
+                orig = getattr(self, c + "_ORIG")
+                setattr(self, c + "CENTER", (np.amax(orig) + np.amin(orig)) / 2.0)
+            self._set_anisotropy([getattr(self, a) for a in self._SCALINGS + self._ANGLES])
+        self._append_drift_data(extra)
+
+        # the variogram stays; the experimental variogram and the statistics belong to the data
+        X, vals = self._stats_inputs()
+        self.lags, self.semivariance, _ = _initialize_variogram_model(
+            X, vals, self.variogram_model, list(self.variogram_model_parameters), self.variogram_function, self._nlags,
+            False, self.coordinates_type, lazy=True)
+        if getattr(self, "_stats_state", "off") == "done":
+            self._stats_state = "lazy"
+
+        self._kb_key = None
+        if getattr(self, "_kb_group", None) is not None:
+            self._kb_gkey = None
+        if fast and getattr(self, "functional_drift", False) and self._anisotropy()[0] != frame:
+            # the callables see the adjusted coordinates: unless the map is the identity, a new centre moves them
+            _, _, _, _, _, Mt = self._data_arrays()
+            fast = np.array_equal(np.asarray(Mt, dtype=float).reshape(self._ndim, self._ndim), np.eye(self._ndim))
+        if fast and self._device_model()[0] == self.TABLE_MODEL_ID:
+            fast = self._table_dmax() == dmax      # a longer table is a new problem
+        if not fast:
+            return
+        _, cols = self._drift_spec()
+        try:
+            h.append_data(*(new[:self._ndim] + [None] * (3 - self._ndim)), new[-1], [np.asarray(c, dtype=np.float64)[-m:] for c in cols] or None)
+        except (NotImplementedError, np.linalg.LinAlgError):
+            return                              # the next execute() sets the problem up from scratch
+        self._kb_key = self._problem_key(key.dtype, False)
+
+    def _new_drift_data(self, coords, m, specified_drift):
+        """Checks the drift data of m new stations before anything changes (the constructor's messages) and returns
+        what _append_drift_data needs: here the 'specified' arrays."""
+        if not getattr(self, "specified_drift", False):
+            if specified_drift:
+                warnings.warn("Provided specified drift values, but 'specified' drift was not initialized during "
+                              "instantiation of %s class." % type(self).__name__, RuntimeWarning)
+            return {}
+        if specified_drift is None:
+            specified_drift = []
+        if type(specified_drift) is not list:
+            raise TypeError("Arrays for specified drift terms must be encapsulated in a list.")
+        if len(specified_drift) == 0:
+            raise ValueError("Must provide at least one drift-value array when using the 'specified' drift capability.")
+        arrays = [np.atleast_1d(np.squeeze(np.array(term, copy=True))) for term in specified_drift]
+        if len(arrays) != len(self.specified_drift_data_arrays):
+            raise ValueError("Inconsistent number of specified drift terms supplied.")
+        if any(a.size != m for a in arrays):
+            raise ValueError("Must specify the drift values for each data point when using the 'specified' drift capability.")
+        return {"specified": arrays}
+
+    def _append_drift_data(self, extra):
+        if "specified" in extra:
+            self.specified_drift_data_arrays = [np.concatenate([np.ravel(old), np.ravel(a)])
+                                                for old, a in zip(self.specified_drift_data_arrays, extra["specified"])]
+
     @staticmethod
     def _check_backend(backend, what):
         if backend != "cuda":
@@ -864,6 +950,32 @@ class Krige2D(KrigeBase):
                                      (anisotropy_scaling, anisotropy_angle))
 
 
+    def add_data(self, x, y, z, specified_drift=None):
+        """Adds stations at (x, y) with values z after the existing ones (monitoring networks that gain stations while
+        the variogram stays). ``specified_drift`` (UniversalKriging with a 'specified' drift term): the list of drift
+        arrays at the new stations, one per array of the constructor; the external_Z, point_log and functional drift
+        values at the new stations are computed as the constructor computes them.
+
+        The variogram is NOT refitted, even for an object built with an automatic fit: the current model and parameters
+        stay, as if a new object were built with them given as fixed parameters. Everything that depends on the data
+        follows the extended data exactly as a new object built on the old stations followed by the new ones (in that
+        order) would: the original and adjusted coordinates, the centre of the anisotropy, the experimental variogram
+        (``lags``, ``semivariance``), the statistics (recomputed on their next access), the drift data and every
+        result of execute(), leave_one_out() and leave_group_out().
+
+        When the handle holds the positive definite global factorisation of this object's current problem (after a
+        global execute() in any dtype, or a cross-validation), the factorisation is extended on the device instead of
+        being redone: one new block row of L and L^-1, about 2 m n^2 flops for m new stations, and the next execute()
+        in the same dtype uses it. Otherwise the stations are only recorded and the next call sets the problem up
+        from scratch, as for a new object: nothing held yet, a moving-window (n_closest_points) problem,
+        ``pseudo_inv=True``, the indefinite fallback (a variogram that is not valid in this dimension), a problem of
+        execute(values=...), ``n_gpus > 1``, a 'custom' variogram whose tabulated range no longer covers the data,
+        'functional' drift terms with anisotropy when the centre moves (the callables see the adjusted coordinates),
+        and an extended matrix that is singular (the new problem then raises as a new object would).
+        """
+        self._add_data((x, y), z, specified_drift)
+
+
 class Krige3D(KrigeBase):
     """OrdinaryKriging3D and UniversalKriging3D: data X_ORIG, Y_ORIG, Z_ORIG with values VALUES."""
     _ndim = 3
@@ -879,3 +991,27 @@ class Krige3D(KrigeBase):
         self._update_variogram_model(variogram_model, variogram_parameters, variogram_function, nlags, weight,
                                      (anisotropy_scaling_y, anisotropy_scaling_z, anisotropy_angle_x,
                                       anisotropy_angle_y, anisotropy_angle_z))
+
+    def add_data(self, x, y, z, val, specified_drift=None):
+        """Adds stations at (x, y, z) with values val after the existing ones; ``specified_drift`` as in
+        UniversalKriging.add_data (UniversalKriging3D with a 'specified' drift term; functional drift values at the new
+        stations are computed as the constructor computes them).
+
+        The variogram is NOT refitted, even for an object built with an automatic fit: the current model and parameters
+        stay, as if a new object were built with them given as fixed parameters. Everything that depends on the data
+        follows the extended data exactly as a new object built on the old stations followed by the new ones (in that
+        order) would: the original and adjusted coordinates, the centre of the anisotropy, the experimental variogram
+        (``lags``, ``semivariance``), the statistics (recomputed on their next access), the drift data and every
+        result of execute(), leave_one_out() and leave_group_out().
+
+        When the handle holds the positive definite global factorisation of this object's current problem (after a
+        global execute() in any dtype, or a cross-validation), the factorisation is extended on the device instead of
+        being redone: one new block row of L and L^-1, about 2 m n^2 flops for m new stations, and the next execute()
+        in the same dtype uses it. Otherwise the stations are only recorded and the next call sets the problem up
+        from scratch, as for a new object: nothing held yet, a moving-window (n_closest_points) problem,
+        ``pseudo_inv=True``, the indefinite fallback (a variogram that is not valid in this dimension), a problem of
+        execute(values=...), ``n_gpus > 1``, a 'custom' variogram whose tabulated range no longer covers the data,
+        'functional' drift terms with anisotropy when the centre moves (the callables see the adjusted coordinates),
+        and an extended matrix that is singular (the new problem then raises as a new object would).
+        """
+        self._add_data((x, y, z), val, specified_drift)

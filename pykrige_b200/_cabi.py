@@ -39,7 +39,7 @@ EXPORTS = [
     "kb200_blob_bytes", "kb200_blob_ptr", "kb200_describe_problem", "kb200_blob_commit",
     "kb200_set_coordinates", "kb200_set_stream", "kb200_last_timings", "kb200_reset_counters", "kb200_debug_fetch",
     "kb200_experimental_variogram", "kb200_statistics", "kb200_loo", "kb200_knn_loo", "kb200_lgo", "kb200_knn_lgo",
-    "kb200_set_pseudo_inverse",
+    "kb200_set_pseudo_inverse", "kb200_append_data",
     "kb200_set_variogram_table", "kb200_set_device_drift", "kb200_set_values",
     "kb200_group_create", "kb200_group_destroy", "kb200_group_last_error", "kb200_group_size", "kb200_group_member",
     "kb200_group_set_problem", "kb200_group_set_problem_knn", "kb200_group_execute_points",
@@ -107,6 +107,7 @@ def load_library():
     lib.kb200_lgo.argtypes = [h, dp, i32, dp, dp]
     lib.kb200_knn_lgo.argtypes = [h, i32, dp, i32, dp, dp]
     lib.kb200_set_pseudo_inverse.argtypes = [h, i32]
+    lib.kb200_append_data.argtypes = [h, i64, dp, dp, dp, dp, dp]
     lib.kb200_set_variogram_table.argtypes = [h, i64, ctypes.c_double, dp]
     lib.kb200_set_device_drift.argtypes = [h, i32, dp, i64, i64, dp, dp, dp]
     lib.kb200_set_values.argtypes = [h, i32, i64, dp]
@@ -450,6 +451,17 @@ class Handle(_Binding):
         z, ss = self._outputs(n)
         self._check(self.lib.kb200_knn_lgo(self._h, int(k), _ptr(g), int(n_groups), _ptr(z), _ptr(ss)), knn=True)
         return z, ss
+
+    def append_data(self, x, y, z, values, drift_cols=None):
+        """The problem set_problem factored on this handle grows by the stations (x, y[, z], values), original
+        coordinates, kept in the held frame (kb200_append_data). drift_cols: the host drift columns at the new stations
+        ([n_hd, m], the order of set_problem's drift_data) or None. NotImplementedError when the held problem has no
+        append form, numpy.linalg.LinAlgError when the extended matrix is singular: the handle then holds no problem."""
+        x, y, z, values = _f64(x), _f64(y), _f64(z), _f64(values)
+        d = None
+        if drift_cols is not None and len(drift_cols):
+            d = _f64(np.asarray(drift_cols, dtype=np.float64).reshape(len(drift_cols), -1))
+        self._check(self.lib.kb200_append_data(self._h, int(x.size), _ptr(x), _ptr(y), _ptr(z), _ptr(values), _ptr(d)))
 
     def debug_fetch(self, what, count):
         out = np.empty(int(count), dtype=np.float64)

@@ -331,7 +331,35 @@ extern "C" int kb200_set_variogram_table(kb200_handle h, int64_t n_nodes, double
     return KB200_OK;
 }
 
+// [lo, hi] grown by the device coordinates of n points: adjusted with the handle's anisotropy (h->an), or the unit
+// vectors of geographic lon/lat
+static void extend_box(const kb200_ctx* h, int dim, int64_t n, const double* x, const double* y, const double* z,
+                       double* lo, double* hi) {
+    for (int64_t i = 0; i < n; ++i) {
+        if (h->geo) {
+            const double rad = 0.017453292519943295;
+            double u[3] = {std::cos(x[i] * rad) * std::cos(y[i] * rad), std::sin(x[i] * rad) * std::cos(y[i] * rad),
+                           std::sin(y[i] * rad)};
+            for (int r = 0; r < 3; ++r) { lo[r] = std::min(lo[r], u[r]); hi[r] = std::max(hi[r], u[r]); }
+            continue;
+        }
+        double d[3] = {x[i] - h->an.c[0], y[i] - h->an.c[1], dim == 3 ? z[i] - h->an.c[2] : 0.0};
+        for (int r = 0; r < dim; ++r) {
+            double v = h->an.c[r];
+            for (int c = 0; c < dim; ++c) v += h->an.m[r * dim + c] * d[c];
+            lo[r] = std::min(lo[r], v); hi[r] = std::max(hi[r], v);
+        }
+    }
+}
+
+static double box_diag2(int sdim, const double* lo, const double* hi) {
+    double diag2 = 0.0;
+    for (int r = 0; r < sdim; ++r) diag2 += (hi[r] - lo[r]) * (hi[r] - lo[r]);
+    return diag2;
+}
+
 // ---- description (shared by set_problem / describe_problem / set_problem_knn) ----
+static int layout(kb200_ctx* h, bool knn_only);
 static int describe(kb200_ctx* h, bool knn_only, int dim, int dtype, int64_t n,
                     const double* x, const double* y, const double* z, const double* values,
                     const double* center, const double* aniso, int model, const double* vparams, int n_vparams,
@@ -394,25 +422,10 @@ static int describe(kb200_ctx* h, bool knn_only, int dim, int dtype, int64_t n,
     // adjusted bounding box on the host (drift rescale + c0 for unbounded models)
     double lo[3] = {1e300, 1e300, 1e300}, hi[3] = {-1e300, -1e300, -1e300};
     const int sdim = h->geo ? 3 : dim;            // spatial dimensions of the device coordinates
-    for (int64_t i = 0; i < n; ++i) {
-        if (h->geo) {
-            const double rad = 0.017453292519943295;
-            double u[3] = {std::cos(x[i] * rad) * std::cos(y[i] * rad), std::sin(x[i] * rad) * std::cos(y[i] * rad),
-                           std::sin(y[i] * rad)};
-            for (int r = 0; r < 3; ++r) { lo[r] = std::min(lo[r], u[r]); hi[r] = std::max(hi[r], u[r]); }
-            continue;
-        }
-        double d[3] = {x[i] - h->an.c[0], y[i] - h->an.c[1], dim == 3 ? z[i] - h->an.c[2] : 0.0};
-        for (int r = 0; r < dim; ++r) {
-            double v = h->an.c[r];
-            for (int c = 0; c < dim; ++c) v += h->an.m[r * dim + c] * d[c];
-            lo[r] = std::min(lo[r], v); hi[r] = std::max(hi[r], v);
-        }
-    }
+    extend_box(h, dim, n, x, y, z, lo, hi);
     if (h->geo) for (int r = 0; r < 3; ++r) { lo[r] -= 1e-9; hi[r] += 1e-9; }   // device sincos may differ in the last ulp
     for (int r = 0; r < 3; ++r) { h->bb_lo[r] = r < sdim ? lo[r] : 0.0; h->bb_hi[r] = r < sdim ? hi[r] : 0.0; }
-    double diag2 = 0.0;
-    for (int r = 0; r < sdim; ++r) diag2 += (hi[r] - lo[r]) * (hi[r] - lo[r]);
+    const double diag2 = box_diag2(sdim, lo, hi);
     if (model == KB200_VG_TABLE && h->tab_dmax < (h->geo ? 180.0 : std::sqrt(diag2)))
         return fail(h, KB200_EBADARG, "variogram table: dmax is smaller than the extent of the data");
     double c0 = host_gamma(h, h->vg, h->geo ? 180.0 : std::sqrt(diag2));
@@ -443,8 +456,15 @@ static int describe(kb200_ctx* h, bool knn_only, int dim, int dtype, int64_t n,
         h->vg.c0 = 0.0;
         for (int c = 0; c <= KB200_MAX_DRIFT; ++c) { h->ds.shift[c] = 0.0; h->ds.scale[c] = 1.0; }
     }
+    int rc = layout(h, knn_only);
+    if (rc) return rc;
+    h->described = true;
+    return KB200_OK;
+}
 
-    // tile stream map
+// Tile stream map and blob layout of a problem of h->n data points; (re)allocates the blob
+static int layout(kb200_ctx* h, bool knn_only) {
+    const int64_t n = h->n;
     h->n_pad = (int)align_up((size_t)n, KB_BM);
     h->ld = h->n_pad;
     h->nrb = knn_only ? 0 : (int)((n + h->na + KB_BM - 1) / KB_BM);
@@ -476,7 +496,6 @@ static int describe(kb200_ctx* h, bool knn_only, int dim, int dtype, int64_t n,
     h->blob_bytes = knn_only ? h->off_tiles : o;
     cudaSetDevice(h->device);
     CU(h, h->blob.reserve(h->blob_bytes));
-    h->described = true;
     return KB200_OK;
 }
 
@@ -588,13 +607,12 @@ static int factor_general(kb200_ctx* h, const BlobView& b, double c0, float* t_c
     return 1;
 }
 
-// C = L L^T (L in wC): W = L^-1, the dual vectors, and W packed into the tiles of the handle's dtype
-static int factor_cholesky_pack(kb200_ctx* h, const BlobView& b, int* launches) {
+// W = L^-1 in wW: the dual vectors, and W packed into the tiles of the handle's dtype
+static int dual_pack(kb200_ctx* h, const BlobView& b, int* launches) {
     cudaStream_t st = h->stream;
     const int nn = h->n, np = h->n_pad, ld = h->ld;
     double* W = h->wW.as<double>();
     double* Uz = aux_block(h, AUX_U);
-    CU(h, kbk_trtri(h->wC.as<double>(), W, h->wT.as<double>(), ld, np, st, launches));
     CU(h, cudaEventRecord(h->ev[EV_DUAL], st));
     CU(h, kbk_dual(W, ld, nn, np, h->n_rl, h->n_hd, h->nf ? h->nf : 1, b.ax, b.ay, b.az, h->ds, raw_col(h, RAW_DRIFT),
                    kriged_values(h), aux_block(h, AUX_F), aux_block(h, AUX_H), Uz, b.consts, h->wFlag.as<int>(), st,
@@ -616,6 +634,12 @@ static int factor_cholesky_pack(kb200_ctx* h, const BlobView& b, int* launches) 
         CU(h, kbk_pack(W, ld, nn, np, h->na, Uz, h->pm, b.tiles, st)); ++*launches;
     }
     return 0;
+}
+
+// C = L L^T (L in wC): W = L^-1, then dual_pack
+static int factor_cholesky_pack(kb200_ctx* h, const BlobView& b, int* launches) {
+    CU(h, kbk_trtri(h->wC.as<double>(), h->wW.as<double>(), h->wT.as<double>(), h->ld, h->n_pad, h->stream, launches));
+    return dual_pack(h, b, launches);
 }
 
 // the high-priority side stream and the ordering events kbk_cholesky needs for a matrix of n_pad rows (kept on the handle)
@@ -704,6 +728,110 @@ extern "C" int kb200_set_problem(kb200_handle h, int dim, int dtype, int64_t n,
     h->ready = true;
     h->local_factor = true;
     return KB200_OK;
+}
+
+// ---- appended stations (DESIGN.md §5g) ----------------------------------------------------------------------------
+// rows and columns [0, keep) of a matrix of stride ld_old into a new allocation of `bytes` with the handle's stride
+static int restride(kb200_ctx* h, DevBuf& b, int ld_old, int keep, size_t bytes) {
+    DevBuf nb;
+    CU(h, nb.reserve(bytes));
+    if (keep > 0)
+        CU(h, cudaMemcpy2DAsync(nb.p, (size_t)h->ld * 8, b.p, (size_t)ld_old * 8, (size_t)keep * 8, keep,
+                                cudaMemcpyDeviceToDevice, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
+    b.release();
+    std::swap(b.p, nb.p); std::swap(b.cap, nb.cap);
+    return KB200_OK;
+}
+
+// The held problem grows by m stations (checked by kb200_append_data). Any error leaves it half-extended: the caller
+// drops it.
+static int append_extend(kb200_ctx* h, int m, const double* x, const double* y, const double* z, const double* values,
+                         const double* drift_cols, const double* lo, const double* hi) {
+    cudaStream_t st = h->stream;
+    const int n_old = h->n, ld_old = h->ld, n0 = n_old / 64 * 64, nn = n_old + m;
+    h->hx.insert(h->hx.end(), x, x + m);
+    h->hy.insert(h->hy.end(), y, y + m);
+    if (h->dim == 3) h->hz.insert(h->hz.end(), z, z + m); else h->hz.resize(nn, 0.0);
+    h->hval.insert(h->hval.end(), values, values + m);
+    if (h->n_hd) {                                    // column-major n x n_hd: each column grows by its m new rows
+        std::vector<double> d((size_t)h->n_hd * nn);
+        for (int c = 0; c < h->n_hd; ++c) {
+            std::copy(h->hdrift.begin() + (size_t)c * n_old, h->hdrift.begin() + (size_t)(c + 1) * n_old, d.begin() + (size_t)c * nn);
+            std::copy(drift_cols + (size_t)c * m, drift_cols + (size_t)(c + 1) * m, d.begin() + (size_t)c * nn + n_old);
+        }
+        h->hdrift.swap(d);
+    }
+    for (int r = 0; r < 3; ++r) { h->bb_lo[r] = lo[r]; h->bb_hi[r] = hi[r]; }
+    h->n = nn;
+    int rc = layout(h, false); if (rc) return rc;
+    const int np = h->n_pad, ld = h->ld;
+    const size_t mat = (size_t)np * ld * sizeof(double);
+    if (ld != ld_old) {                               // n_pad grew: L11 and W11 move to the new stride
+        rc = restride(h, h->wC, ld_old, n0, mat); if (rc) return rc;
+        rc = restride(h, h->wW, ld_old, n0, mat); if (rc) return rc;
+    }
+    CU(h, h->wT.reserve(mat));
+    CU(h, h->wF.reserve((size_t)3 * h->aux_cols * np * sizeof(double)));
+    const BlobView b = blob_view(h);
+    int* flag = h->wFlag.as<int>();
+    int launches = 0;
+    rc = upload_data(h, true, &launches); if (rc) return rc;
+    rc = cholesky_streams(h, np - n0); if (rc) return rc;
+    CU(h, cudaMemsetAsync(flag, 0, sizeof(int), st));
+    CU(h, cudaEventRecord(h->ev[EV_ASM], st));
+    CU(h, kbk_assemble_rows(h->dim, h->vg, nn, np, ld, n0 / 64, b.ax, b.ay, b.az, h->wC.as<double>(), st)); ++launches;
+    CU(h, cudaEventRecord(h->ev[EV_FACTOR], st));
+    CU(h, kbk_append_factor(h->wC.as<double>(), h->wW.as<double>(), h->wT.as<double>(), ld, np, n0, flag,
+                            3.6e-15 * h->vg.c0, st, h->hi_stream, h->fev.data(), (int)h->fev.size(), &launches));
+    CU(h, cudaEventRecord(h->ev[EV_INVERT], st));
+    int hflag = 0;
+    CU(h, cudaMemcpyAsync(&hflag, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    h->tm[TM_H2D] += ev_ms(h->ev[EV_UPLOAD], h->ev[EV_ADJUSTED]);
+    h->tm[TM_ASSEMBLE] += ev_ms(h->ev[EV_ASM], h->ev[EV_FACTOR]);
+    h->tm[TM_CHOLESKY] += ev_ms(h->ev[EV_FACTOR], h->ev[EV_INVERT]);
+    if (hflag != 0) {
+        h->launches += launches;
+        return fail(h, KB200_ESINGULAR, "kriging matrix is singular (zero pivot in column " + std::to_string(n0 + hflag - 1) + ")");
+    }
+    CU(h, cudaMemsetAsync(b.consts, 0, (size_t)std::max(512, h->K1 * h->na) * sizeof(double), st));
+    rc = dual_pack(h, b, &launches); if (rc) return rc;
+    double hdr[HDR_DOUBLES];
+    write_header(h, hdr);
+    CU(h, cudaMemcpyAsync(b.hdr, hdr, sizeof(hdr), cudaMemcpyHostToDevice, st));
+    CU(h, cudaEventRecord(h->ev[EV_PACKED], st));
+    CU(h, cudaMemcpyAsync(&hflag, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    h->tm[TM_PACK_DUAL] += ev_ms(h->ev[EV_DUAL], h->ev[EV_PACKED]);
+    h->launches += launches;
+    if (hflag != 0) return fail(h, KB200_ESINGULAR, "drift/unbiasedness block F^T C^-1 F is singular");
+    return KB200_OK;
+}
+
+extern "C" int kb200_append_data(kb200_handle h, int64_t m, const double* x, const double* y, const double* z,
+                                 const double* values, const double* drift_cols) {
+    if (!h) return KB200_EBADARG;
+    if (!h->ready || !h->local_factor)
+        return fail(h, KB200_EUNSUPPORTED, "append: no global problem was factored on this handle");
+    if (h->gform != 0)
+        return fail(h, KB200_EUNSUPPORTED, "append: the held problem is not a positive definite covariance form "
+                    "(pseudo-inverse or the indefinite fallback)");
+    if (h->nf) return fail(h, KB200_EUNSUPPORTED, "append: value fields (kb200_set_values) have no append form");
+    const int dim = h->dim == 3 ? 3 : 2;
+    if (m < 1 || !x || !y || (dim == 3 && !z) || !values || (h->n_hd && !drift_cols))
+        return fail(h, KB200_EBADARG, "append: m >= 1 and non-null arrays (drift_cols with drift columns)");
+    if (h->n + m > (int64_t)(KB_MAXRB - 1) * KB_BM) return fail(h, KB200_EBADARG, "n out of range");
+    double lo[3], hi[3];
+    for (int r = 0; r < 3; ++r) { lo[r] = h->bb_lo[r]; hi[r] = h->bb_hi[r]; }
+    const int sdim = h->geo ? 3 : dim;
+    extend_box(h, dim, m, x, y, z, lo, hi);
+    if (h->vg.model == KB200_VG_TABLE && h->tab_dmax < (h->geo ? 180.0 : std::sqrt(box_diag2(sdim, lo, hi))))
+        return fail(h, KB200_EUNSUPPORTED, "append: the variogram table's dmax does not cover the extended data");
+    cudaSetDevice(h->device);
+    const int rc = append_extend(h, (int)m, x, y, z, values, drift_cols, lo, hi);
+    if (rc) drop_problem(h);
+    return rc;
 }
 
 // ---- device-evaluated drift terms -----------------------------------------------------------------------

@@ -69,6 +69,45 @@ __global__ void __launch_bounds__(256) assemble_kernel(VgParams vg, int n, int n
     }
 }
 
+// the lower tiles of the tile rows [it0, n_pad / 64) only (kbk_append_factor: the new block row). The tile body is
+// assemble_kernel's, kept as its own copy so that the fresh assembly compiles exactly as before.
+template <int DIM, int MODEL>
+__global__ void __launch_bounds__(256) assemble_rows_kernel(VgParams vg, int n, int ld, int it0,
+                                                             const double* __restrict__ ax,
+                                                             const double* __restrict__ ay,
+                                                             const double* __restrict__ az,
+                                                             double* __restrict__ C) {
+    const int it = it0 + blockIdx.y, jt = blockIdx.x;
+    if (jt > it) return;
+    __shared__ double sx[64], sy[64], sz[64];   // column (j) points
+    int tid = threadIdx.x;
+    if (tid < 64) {
+        int j = jt * 64 + tid;
+        bool ok = j < n;
+        sx[tid] = ok ? ax[j] : 0.0;
+        sy[tid] = ok ? ay[j] : 0.0;
+        sz[tid] = (ok && KB_HASZ(DIM)) ? az[j] : 0.0;
+    }
+    __syncthreads();
+    int jl = tid & 63;          // column within tile (contiguous -> coalesced stores)
+    int i0 = tid >> 6;          // 0..3
+    int j = jt * 64 + jl;
+    for (int r = i0; r < 64; r += 4) {
+        int i = it * 64 + r;
+        double v;
+        if (i < n && j < n) {
+            if (i == j) v = vg.c0;
+            else {
+                double d = kb_dist<DIM>(ax[i], ay[i], KB_HASZ(DIM) ? az[i] : 0.0, sx[jl], sy[jl], sz[jl]);
+                v = vg.c0 - kb_gamma<MODEL>(vg, d);
+            }
+        } else {
+            v = (i == j) ? 1.0 : 0.0;
+        }
+        C[(size_t)i * ld + j] = v;
+    }
+}
+
 // ---------------------------------------------------------------------------
 // 64x64 DMMA GEMM tile core used by the Cholesky trailing update, the
 // triangular inverse and the Gram product W^T W: acc(64x64) += A(64 x [k0,k1)) * B([k0,k1) x 64).
@@ -466,6 +505,32 @@ __global__ void __launch_bounds__(128) gram_lower_kernel(const double* __restric
 }
 
 // ---------------------------------------------------------------------------
+// Appended stations (kb200_append_data, DESIGN.md §5g): the block row [n0, n_pad) of L and W from the held L11, W11 of
+// rows [0, n0). One 64x64 output tile (ti, tj) per CTA; the k range of each product skips the zero triangle of its
+// triangular factor:
+//   AP_L21   L21 = C21 W11^T        (NT)  W11[j][k] = 0 for k > j
+//   AP_SYRK  S   = C22 - L21 L21^T  (NT)  lower tiles only, k over [0, n0)
+//   AP_T     T   = L21 W11          (NN)  W11[k][j] = 0 for k < j
+//   AP_W21   W21 = -W22 T           (NN)  W22[i][k] = 0 for k > i
+// A, B and out point at the first row (and, for NN-B / out, column) of their blocks; all share the stride ld.
+enum AppendGemm { AP_L21 = 0, AP_SYRK = 1, AP_T = 2, AP_W21 = 3 };
+template <bool NT>
+__global__ void __launch_bounds__(128) append_gemm_kernel(const double* __restrict__ A, const double* __restrict__ B,
+                                                          double* __restrict__ out, int ld, int kend, int mode,
+                                                          double alpha, double beta) {
+    __shared__ GemmSmem sm;
+    const int tj = blockIdx.x, ti = blockIdx.y;
+    int k0 = 0, k1 = kend;
+    if (mode == AP_L21) k1 = (tj + 1) * 64;
+    else if (mode == AP_SYRK) { if (tj > ti) return; }
+    else if (mode == AP_T) k0 = tj * 64;
+    else k1 = (ti + 1) * 64;
+    double acc[4][4][2] = {};
+    gemm_tile_64<NT>(acc, sm, A + (size_t)ti * 64 * ld, ld, NT ? B + (size_t)tj * 64 * ld : B + tj * 64, ld, k0, k1);
+    gemm_tile_store(acc, out + (size_t)ti * 64 * ld + tj * 64, ld, alpha, beta);
+}
+
+// ---------------------------------------------------------------------------
 // K2c  dual vectors.  Fz (n x na, column-major, column stride n_pad) holds the drift
 // columns, the ones column and the data values.  Hz = W Fz ; Uz = W^T Hz = C^-1 Fz.
 // Regional-linear columns are built on device from the adjusted coordinates
@@ -717,6 +782,43 @@ cudaError_t kbk_trtri(const double* L, double* W, double* T1, int ld, int n_pad,
         dim3 grid(m / 64, m / 64, pairs);
         trtri_step1_kernel<<<grid, 128, 0, st>>>(L, W, T1, ld, n_pad, m);
         trtri_step2_kernel<<<grid, 128, 0, st>>>(W, T1, ld, n_pad, m);
+        *launches += 2;
+    }
+    return cudaGetLastError();
+}
+
+cudaError_t kbk_assemble_rows(int dim, const VgParams& vg, int n, int n_pad, int ld, int it0,
+                              const double* ax, const double* ay, const double* az, double* C, cudaStream_t st) {
+    const int nb = n_pad / 64;
+    return KbDims::dispatch(dim, [&](auto D) {
+        return KbModels::dispatch(vg.model, [&](auto M) {
+            assemble_rows_kernel<D, M><<<dim3(nb, nb - it0), 256, 0, st>>>(vg, n, ld, it0, ax, ay, az, C);
+            return cudaGetLastError();
+        });
+    });
+}
+
+// L21 = C21 W11^T, S = C22 - L21 L21^T, L22 = chol(S), W22 = L22^-1 (the panel chain and level-doubling inverse of a
+// fresh factorisation, on the corner), W21 = -W22 (L21 W11). T is scratch of C's shape: L21 waits there until the Schur
+// complement has read it, then the corner's staged diagonal factors and T1 of the inverse, then T = L21 W11.
+cudaError_t kbk_append_factor(double* C, double* W, double* T, int ld, int n_pad, int n0, int* flag, double dtol,
+                              cudaStream_t st, cudaStream_t hi, cudaEvent_t* ev, int n_ev, int* launches) {
+    const int nb0 = n0 / 64, nbr = (n_pad - n0) / 64;
+    const size_t r0 = (size_t)n0 * ld;
+    double* C22 = C + r0 + n0;
+    double* W22 = W + r0 + n0;
+    if (nb0 > 0) {
+        append_gemm_kernel<true><<<dim3(nb0, nbr), 128, 0, st>>>(C + r0, W, T + r0, ld, n0, AP_L21, 1.0, 0.0);
+        append_gemm_kernel<true><<<dim3(nbr, nbr), 128, 0, st>>>(T + r0, T + r0, C22, ld, n0, AP_SYRK, -1.0, 1.0);
+        KB_CUDA_OK(cudaMemcpy2DAsync(C + r0, (size_t)ld * 8, T + r0, (size_t)ld * 8, (size_t)n0 * 8, n_pad - n0,
+                                     cudaMemcpyDeviceToDevice, st));
+        *launches += 2;
+    }
+    KB_CUDA_OK(kbk_cholesky(C22, W22, T, ld, n_pad - n0, flag, dtol, st, hi, ev, n_ev, launches));
+    KB_CUDA_OK(kbk_trtri(C22, W22, T + r0 + n0, ld, n_pad - n0, st, launches));
+    if (nb0 > 0) {
+        append_gemm_kernel<false><<<dim3(nb0, nbr), 128, 0, st>>>(C + r0, W, T + r0, ld, n0, AP_T, 1.0, 0.0);
+        append_gemm_kernel<false><<<dim3(nb0, nbr), 128, 0, st>>>(W22, T + r0, W + r0, ld, 0, AP_W21, -1.0, 0.0);
         *launches += 2;
     }
     return cudaGetLastError();

@@ -81,6 +81,7 @@ class UniversalKriging(Krige2D):
             self.point_log_array = np.zeros(point_log.shape)
             self.point_log_array[:, 2] = point_log[:, 2]
             self.point_log_array[:, :2] = self._adjust(point_log[:, 0], point_log[:, 1]).T
+            self._point_log_orig = point_log[:, :2].copy()      # the wells move with the adjusted frame (add_data)
             if self.verbose:
                 print("Implementing external point-logarithmic drift; number of points =",
                       self.point_log_array.shape[0], "\n")
@@ -88,6 +89,21 @@ class UniversalKriging(Krige2D):
             self.point_log_drift = False
 
         self._init_host_drift_terms(drift_terms, specified_drift, functional_drift)
+
+    def _new_drift_data(self, coords, m, specified_drift):
+        extra = super()._new_drift_data(coords, m, specified_drift)
+        if self.external_Z_drift:       # the constructor's domain check, before anything changes
+            extra["z_scalars"] = self._calculate_data_point_zscalars(coords[0], coords[1])
+        return extra
+
+    def _append_drift_data(self, extra):
+        super()._append_drift_data(extra)
+        if "z_scalars" in extra:
+            self.z_scalars = np.concatenate([np.ravel(self.z_scalars), extra["z_scalars"]])
+        if self.point_log_drift:        # as the constructor places the wells, in the moved frame
+            wells = self.point_log_array.copy()
+            wells[:, :2] = self._adjust(self._point_log_orig[:, 0], self._point_log_orig[:, 1]).T
+            self.point_log_array = wells
 
     def _calculate_data_point_zscalars(self, x, y, type_="array"):
         """Bilinear sample of the external-Z grid at (x, y) (uk.py:512-628), vectorised; node
