@@ -558,11 +558,15 @@ static int factor_pinv(kb200_ctx* h, const BlobView& b, int* launches) {
     double* Uz = aux_block(h, AUX_U);
     int* flag = h->wFlag.as<int>();
     CU(h, h->wVario.reserve(kbk_pinv_workspace_doubles(nt) * sizeof(double)));
+    CU(h, cudaMemsetAsync(flag, 0, sizeof(int), st));
+    CU(h, cudaEventRecord(h->ev[EV_ASM], st));
+    CU(h, kbk_assemble(h->dim, h->vg, nn, np, h->ld, 0, b.ax, b.ay, b.az, h->wC.as<double>(), st)); ++*launches;
     CU(h, cudaEventRecord(h->ev[EV_INVERT], st));
     CU(h, kbk_build_fz(nn, np, h->n_rl, h->n_hd, b.ax, b.ay, b.az, h->ds, raw_col(h, RAW_DRIFT), raw_col(h, RAW_V), Fz,
                        st)); ++*launches;
     CU(h, kbk_pinv(nn, h->K1, np, h->wC.as<double>(), h->ld, Fz, raw_col(h, RAW_V), Uz, b.consts, h->wVario.as<double>(),
                    flag, st, launches, &h->pinv_sweeps, &h->pinv_rank));
+    h->tm[TM_ASSEMBLE] += ev_ms(h->ev[EV_ASM], h->ev[EV_INVERT]);     // kbk_pinv ends in a synchronise
     if (h->pinv_sweeps < 0) { h->launches += *launches; return fail(h, KB200_ESINGULAR, "pseudo-inverse: the Jacobi SVD did not converge"); }
     CU(h, cudaMemsetAsync(flag, 0, sizeof(int), st));
     CU(h, cudaEventRecord(h->ev[EV_DUAL], st));
@@ -573,7 +577,7 @@ static int factor_pinv(kb200_ctx* h, const BlobView& b, int* launches) {
 // C is not positive definite: the variogram is not conditionally negative definite in this dimension (e.g. hole-effect
 // on dense scatter). General fallback, from the unshifted c0: blocked Gauss-Jordan inverse with partial pivoting +
 // quadratic-form solve (DESIGN.md §3b). fp64 only.
-static int factor_general(kb200_ctx* h, const BlobView& b, double c0, float* t_chol, int* launches) {
+static int factor_general(kb200_ctx* h, const BlobView& b, double c0, int* launches) {
     if (h->dtype != KB200_F64) {
         h->launches += *launches;
         return fail(h, KB200_EUNSUPPORTED, "dtype float32 / float64x need a positive definite covariance form "
@@ -586,14 +590,14 @@ static int factor_general(kb200_ctx* h, const BlobView& b, double c0, float* t_c
     h->vg.c0 = c0;
     CU(h, cudaMemsetAsync(flag, 0, sizeof(int), st));
     CU(h, cudaEventRecord(h->ev[EV_FACTOR], st));
-    CU(h, kbk_assemble(h->dim, h->vg, nn, np, ld, b.ax, b.ay, b.az, G, st)); ++*launches;
+    CU(h, kbk_assemble(h->dim, h->vg, nn, np, ld, 0, b.ax, b.ay, b.az, G, st)); ++*launches;
     CU(h, h->wVario.reserve(kbk_general_inverse_workspace_bytes(np)));
     CU(h, kbk_general_inverse(G, ld, np, h->wVario.p, flag, 3.6e-15 * h->vg.c0, st, launches));
     CU(h, cudaEventRecord(h->ev[EV_INVERT], st));
     int hflag = 0;
     CU(h, cudaMemcpyAsync(&hflag, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
     CU(h, cudaStreamSynchronize(st));
-    *t_chol += ev_ms(h->ev[EV_FACTOR], h->ev[EV_INVERT]);
+    h->tm[TM_CHOLESKY] += ev_ms(h->ev[EV_FACTOR], h->ev[EV_INVERT]);
     if (hflag != 0) {
         h->launches += *launches;
         return fail(h, KB200_ESINGULAR, "kriging matrix is singular (zero pivot in column " +
@@ -636,13 +640,14 @@ static int dual_pack(kb200_ctx* h, const BlobView& b, int* launches) {
     return 0;
 }
 
-// C = L L^T (L in wC): W = L^-1, then dual_pack
-static int factor_cholesky_pack(kb200_ctx* h, const BlobView& b, int* launches) {
-    CU(h, kbk_trtri(h->wC.as<double>(), h->wW.as<double>(), h->wT.as<double>(), h->ld, h->n_pad, h->stream, launches));
+// C = L L^T (L in wC): W = L^-1 of the rows [n0, n_pad), then dual_pack
+static int factor_cholesky_pack(kb200_ctx* h, const BlobView& b, int n0, int* launches) {
+    CU(h, kbk_inverse_rows(h->wC.as<double>(), h->wW.as<double>(), h->wT.as<double>(), h->ld, h->n_pad, n0, h->stream,
+                           launches));
     return dual_pack(h, b, launches);
 }
 
-// the high-priority side stream and the ordering events kbk_cholesky needs for a matrix of n_pad rows (kept on the handle)
+// the high-priority side stream and the ordering events kbk_cholesky_rows needs for n_pad rows (kept on the handle)
 static int cholesky_streams(kb200_ctx* h, int n_pad) {
     if (!h->hi_stream) {
         int lo = 0, hi = 0;
@@ -658,6 +663,50 @@ static int cholesky_streams(kb200_ctx* h, int n_pad) {
     return KB200_OK;
 }
 
+// Assembles the rows [n0, n_pad) of C with the handle's c0 and factors them (kbk_cholesky_rows; n0 = 0 for a new
+// problem). Returns the pivot flag (0, or 1 + the column of a non-positive pivot counted from n0) or an error code < 0.
+static int assemble_cholesky(kb200_ctx* h, const BlobView& b, int n0, int* launches) {
+    cudaStream_t st = h->stream;
+    const int np = h->n_pad, ld = h->ld;
+    int* flag = h->wFlag.as<int>();
+    const int rc = cholesky_streams(h, np - n0); if (rc) return rc;
+    CU(h, cudaMemsetAsync(flag, 0, sizeof(int), st));
+    CU(h, cudaEventRecord(h->ev[EV_ASM], st));
+    CU(h, kbk_assemble(h->dim, h->vg, h->n, np, ld, n0 / 64, b.ax, b.ay, b.az, h->wC.as<double>(), st)); ++*launches;
+    CU(h, cudaEventRecord(h->ev[EV_FACTOR], st));
+    CU(h, kbk_cholesky_rows(h->wC.as<double>(), h->wW.as<double>(), h->wT.as<double>(), ld, np, n0, flag,
+                            3.6e-15 * h->vg.c0, st, h->hi_stream, h->fev.data(), (int)h->fev.size(), launches));
+    CU(h, cudaEventRecord(h->ev[EV_INVERT], st));
+    int hflag = 0;
+    CU(h, cudaMemcpyAsync(&hflag, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    h->tm[TM_ASSEMBLE] += ev_ms(h->ev[EV_ASM], h->ev[EV_FACTOR]);
+    h->tm[TM_CHOLESKY] += ev_ms(h->ev[EV_FACTOR], h->ev[EV_INVERT]);
+    return hflag;
+}
+
+// The end of every global set-up, after the dual vectors and the pack: the header, the flag of the drift block, the
+// timings and launches of the call. The handle then holds the problem.
+static int finish_problem(kb200_ctx* h, const BlobView& b, int gform, int launches) {
+    cudaStream_t st = h->stream;
+    h->gform = gform;
+    double hdr[HDR_DOUBLES];
+    write_header(h, hdr);
+    CU(h, cudaMemcpyAsync(b.hdr, hdr, sizeof(hdr), cudaMemcpyHostToDevice, st));
+    CU(h, cudaEventRecord(h->ev[EV_PACKED], st));
+    int hflag = 0;
+    CU(h, cudaMemcpyAsync(&hflag, h->wFlag.as<int>(), sizeof(int), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    h->tm[TM_H2D] += ev_ms(h->ev[EV_UPLOAD], h->ev[EV_ADJUSTED]);
+    h->tm[TM_TRTRI] += ev_ms(h->ev[EV_INVERT], h->ev[EV_DUAL]);
+    h->tm[TM_PACK_DUAL] += ev_ms(h->ev[EV_DUAL], h->ev[EV_PACKED]);
+    h->launches += launches;
+    if (hflag != 0) return fail(h, KB200_ESINGULAR, "drift/unbiasedness block F^T C^-1 F is singular");
+    h->ready = true;
+    h->local_factor = true;
+    return KB200_OK;
+}
+
 extern "C" int kb200_set_problem(kb200_handle h, int dim, int dtype, int64_t n,
                                  const double* x, const double* y, const double* z, const double* values,
                                  const double* center, const double* aniso,
@@ -666,68 +715,35 @@ extern "C" int kb200_set_problem(kb200_handle h, int dim, int dtype, int64_t n,
     int rc = describe(h, false, dim, dtype, n, x, y, z, values, center, aniso, model, vparams, n_vparams,
                       exact_values, eps, n_rl, n_hd, drift_data);
     if (rc != KB200_OK) return rc;
-    cudaStream_t st = h->stream;
-    const int np = h->n_pad, ld = h->ld, nn = h->n;
+    const int np = h->n_pad, ld = h->ld;
     const size_t mat = (size_t)np * ld * sizeof(double);
     CU(h, h->wC.reserve(mat)); CU(h, h->wW.reserve(mat)); CU(h, h->wT.reserve(mat));
     CU(h, h->wF.reserve((size_t)3 * h->aux_cols * np * sizeof(double)));
     CU(h, h->wFlag.reserve(256));
     const BlobView b = blob_view(h);
-    int* flag = h->wFlag.as<int>();
     int launches = 0;
     rc = upload_data(h, true, &launches); if (rc) return rc;
 
     // covariance shift: c0 = sill for bounded models; for linear/power grow c0 until C is
     // positive definite (DESIGN.md §3). A model that is not a valid variogram in this
-    // dimension (e.g. hole-effect in 2-D/3-D) never becomes positive definite.
+    // dimension (e.g. hole-effect in 2-D/3-D) never becomes positive definite. pseudo_inv=True
+    // factors nothing: the pseudo-inverse works on -Gamma itself.
     const bool unbounded = (h->vg.model == KB200_VG_LINEAR || h->vg.model == KB200_VG_POWER || h->vg.model == KB200_VG_TABLE);
     const int max_try = unbounded ? 5 : 1;
     const double c0_first = h->vg.c0;
     int hflag = 0;
-    float t_asm = 0.f, t_chol = 0.f;
-    for (int attempt = 0; attempt < max_try; ++attempt) {
-        CU(h, cudaMemsetAsync(flag, 0, sizeof(int), st));
-        CU(h, cudaEventRecord(h->ev[EV_ASM], st));
-        CU(h, kbk_assemble(h->dim, h->vg, nn, np, ld, b.ax, b.ay, b.az, h->wC.as<double>(), st)); ++launches;
-        CU(h, cudaEventRecord(h->ev[EV_FACTOR], st));
-        if (h->pinv) {                                  // no factorisation: the pseudo-inverse works on -Gamma itself
-            CU(h, cudaEventRecord(h->ev[EV_INVERT], st));
-            CU(h, cudaStreamSynchronize(st));
-            t_asm += ev_ms(h->ev[EV_ASM], h->ev[EV_FACTOR]);
-            break;
-        }
-        rc = cholesky_streams(h, np); if (rc) return rc;
-        CU(h, kbk_cholesky(h->wC.as<double>(), h->wW.as<double>(), h->wT.as<double>(), ld, np, flag, 3.6e-15 * h->vg.c0, st, h->hi_stream,
-                           h->fev.data(), (int)h->fev.size(), &launches));
-        CU(h, cudaEventRecord(h->ev[EV_INVERT], st));
-        CU(h, cudaMemcpyAsync(&hflag, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
-        CU(h, cudaStreamSynchronize(st));
-        t_asm += ev_ms(h->ev[EV_ASM], h->ev[EV_FACTOR]); t_chol += ev_ms(h->ev[EV_FACTOR], h->ev[EV_INVERT]);
+    for (int attempt = 0; !h->pinv && attempt < max_try; ++attempt) {
+        hflag = assemble_cholesky(h, b, 0, &launches); if (hflag < 0) return hflag;
         if (hflag != 0 && std::getenv("KB200_DEBUG")) std::fprintf(stderr, "[kb200] cholesky flag %d (attempt %d, c0 %g)\n", hflag, attempt, h->vg.c0);
         if (hflag == 0) break;
         h->vg.c0 *= 2.0;
     }
-    CU(h, cudaMemsetAsync(b.consts, 0, (size_t)std::max(512, h->K1 * h->na) * sizeof(double), st));
+    CU(h, cudaMemsetAsync(b.consts, 0, (size_t)std::max(512, h->K1 * h->na) * sizeof(double), h->stream));
     const int gform = h->pinv ? factor_pinv(h, b, &launches)
-                    : hflag ? factor_general(h, b, c0_first, &t_chol, &launches)
-                    : factor_cholesky_pack(h, b, &launches);
+                    : hflag ? factor_general(h, b, c0_first, &launches)
+                    : factor_cholesky_pack(h, b, 0, &launches);
     if (gform < 0) return gform;
-    h->gform = gform;
-    double hdr[HDR_DOUBLES];
-    write_header(h, hdr);
-    CU(h, cudaMemcpyAsync(b.hdr, hdr, sizeof(hdr), cudaMemcpyHostToDevice, st));
-    CU(h, cudaEventRecord(h->ev[EV_PACKED], st));
-    CU(h, cudaMemcpyAsync(&hflag, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CU(h, cudaStreamSynchronize(st));
-    h->tm[TM_H2D] += ev_ms(h->ev[EV_UPLOAD], h->ev[EV_ADJUSTED]);
-    h->tm[TM_ASSEMBLE] += t_asm; h->tm[TM_CHOLESKY] += t_chol;
-    h->tm[TM_TRTRI] += ev_ms(h->ev[EV_INVERT], h->ev[EV_DUAL]);
-    h->tm[TM_PACK_DUAL] += ev_ms(h->ev[EV_DUAL], h->ev[EV_PACKED]);
-    h->launches += launches;
-    if (hflag != 0) return fail(h, KB200_ESINGULAR, "drift/unbiasedness block F^T C^-1 F is singular");
-    h->ready = true;
-    h->local_factor = true;
-    return KB200_OK;
+    return finish_problem(h, b, gform, launches);
 }
 
 // ---- appended stations (DESIGN.md §5g) ----------------------------------------------------------------------------
@@ -744,11 +760,10 @@ static int restride(kb200_ctx* h, DevBuf& b, int ld_old, int keep, size_t bytes)
     return KB200_OK;
 }
 
-// The held problem grows by m stations (checked by kb200_append_data). Any error leaves it half-extended: the caller
-// drops it.
+// The held problem grows by m stations (checked by kb200_append_data): the set-up of kb200_set_problem on the rows
+// [n0, n_pad), n0 = the old n rounded down to the tile. Any error leaves it half-extended: the caller drops it.
 static int append_extend(kb200_ctx* h, int m, const double* x, const double* y, const double* z, const double* values,
                          const double* drift_cols, const double* lo, const double* hi) {
-    cudaStream_t st = h->stream;
     const int n_old = h->n, ld_old = h->ld, n0 = n_old / 64 * 64, nn = n_old + m;
     h->hx.insert(h->hx.end(), x, x + m);
     h->hy.insert(h->hy.end(), y, y + m);
@@ -774,39 +789,16 @@ static int append_extend(kb200_ctx* h, int m, const double* x, const double* y, 
     CU(h, h->wT.reserve(mat));
     CU(h, h->wF.reserve((size_t)3 * h->aux_cols * np * sizeof(double)));
     const BlobView b = blob_view(h);
-    int* flag = h->wFlag.as<int>();
     int launches = 0;
     rc = upload_data(h, true, &launches); if (rc) return rc;
-    rc = cholesky_streams(h, np - n0); if (rc) return rc;
-    CU(h, cudaMemsetAsync(flag, 0, sizeof(int), st));
-    CU(h, cudaEventRecord(h->ev[EV_ASM], st));
-    CU(h, kbk_assemble_rows(h->dim, h->vg, nn, np, ld, n0 / 64, b.ax, b.ay, b.az, h->wC.as<double>(), st)); ++launches;
-    CU(h, cudaEventRecord(h->ev[EV_FACTOR], st));
-    CU(h, kbk_append_factor(h->wC.as<double>(), h->wW.as<double>(), h->wT.as<double>(), ld, np, n0, flag,
-                            3.6e-15 * h->vg.c0, st, h->hi_stream, h->fev.data(), (int)h->fev.size(), &launches));
-    CU(h, cudaEventRecord(h->ev[EV_INVERT], st));
-    int hflag = 0;
-    CU(h, cudaMemcpyAsync(&hflag, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CU(h, cudaStreamSynchronize(st));
-    h->tm[TM_H2D] += ev_ms(h->ev[EV_UPLOAD], h->ev[EV_ADJUSTED]);
-    h->tm[TM_ASSEMBLE] += ev_ms(h->ev[EV_ASM], h->ev[EV_FACTOR]);
-    h->tm[TM_CHOLESKY] += ev_ms(h->ev[EV_FACTOR], h->ev[EV_INVERT]);
+    const int hflag = assemble_cholesky(h, b, n0, &launches); if (hflag < 0) return hflag;
     if (hflag != 0) {
         h->launches += launches;
         return fail(h, KB200_ESINGULAR, "kriging matrix is singular (zero pivot in column " + std::to_string(n0 + hflag - 1) + ")");
     }
-    CU(h, cudaMemsetAsync(b.consts, 0, (size_t)std::max(512, h->K1 * h->na) * sizeof(double), st));
-    rc = dual_pack(h, b, &launches); if (rc) return rc;
-    double hdr[HDR_DOUBLES];
-    write_header(h, hdr);
-    CU(h, cudaMemcpyAsync(b.hdr, hdr, sizeof(hdr), cudaMemcpyHostToDevice, st));
-    CU(h, cudaEventRecord(h->ev[EV_PACKED], st));
-    CU(h, cudaMemcpyAsync(&hflag, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CU(h, cudaStreamSynchronize(st));
-    h->tm[TM_PACK_DUAL] += ev_ms(h->ev[EV_DUAL], h->ev[EV_PACKED]);
-    h->launches += launches;
-    if (hflag != 0) return fail(h, KB200_ESINGULAR, "drift/unbiasedness block F^T C^-1 F is singular");
-    return KB200_OK;
+    CU(h, cudaMemsetAsync(b.consts, 0, (size_t)std::max(512, h->K1 * h->na) * sizeof(double), h->stream));
+    rc = factor_cholesky_pack(h, b, n0, &launches); if (rc) return rc;
+    return finish_problem(h, b, 0, launches);
 }
 
 extern "C" int kb200_append_data(kb200_handle h, int64_t m, const double* x, const double* y, const double* z,
@@ -1800,9 +1792,9 @@ extern "C" int kb200_lgo(kb200_handle h, const int32_t* group, int n_groups, dou
             CU(h, cudaMemsetAsync(flag, 0, sizeof(int), st));
             CU(h, kbk_lgo_pad(blk + boff[g], m, A, gp, smax, st)); ++launches;
             if (h->gform == 0) {
-                CU(h, kbk_cholesky(A, Wm, T1, gp, gp, flag, KB_LOO_TOL * smax, st, h->hi_stream, h->fev.data(),
-                                   (int)h->fev.size(), &launches));
-                CU(h, kbk_trtri(A, Wm, T1, gp, gp, st, &launches));
+                CU(h, kbk_cholesky_rows(A, Wm, T1, gp, gp, 0, flag, KB_LOO_TOL * smax, st, h->hi_stream, h->fev.data(),
+                                        (int)h->fev.size(), &launches));
+                CU(h, kbk_inverse_rows(A, Wm, T1, gp, gp, 0, st, &launches));
                 CU(h, kbk_gram_lower(Wm, gp, gp, A, gp, st)); ++launches;
             } else {
                 CU(h, kbk_general_inverse(A, gp, gp, h->wVario.p, flag, KB_LOO_TOL * smax, st, &launches));

@@ -26,59 +26,21 @@ __global__ void adjust_data_kernel(Aniso an, int n, const double* __restrict__ x
 
 // ---------------------------------------------------------------------------
 // K1: C[i][j] = c0 - gamma(|p_i - p_j|) (i != j), c0 on the diagonal; identity in the
-// padding. Only tiles on/below the diagonal are written (Cholesky reads the lower triangle).
+// padding. Only tiles on/below the diagonal are written (Cholesky reads the lower triangle), and only those of the
+// tile rows [it0, n_pad / 64): it0 = 0 for a new factorisation, the first new tile row for appended stations.
 // HBM-write bound: n_pad^2/2 * 8 bytes.
 template <int DIM, int MODEL>
-__global__ void __launch_bounds__(256) assemble_kernel(VgParams vg, int n, int n_pad, int ld,
+__global__ void __launch_bounds__(256) assemble_kernel(VgParams vg, int n, int ld, int it0,
                                                         const double* __restrict__ ax,
                                                         const double* __restrict__ ay,
                                                         const double* __restrict__ az,
                                                         double* __restrict__ C) {
-    // blockIdx.x -> lower-triangular tile (it >= jt) of 64x64
-    int t = blockIdx.x;
+    // blockIdx.x -> lower-triangular tile (it >= jt) of 64x64, counted from the first tile of row it0
+    int t = blockIdx.x + it0 * (it0 + 1) / 2;
     int it = (int)((sqrt(8.0 * (double)t + 1.0) - 1.0) * 0.5);
     while ((long long)(it + 1) * (it + 2) / 2 <= t) ++it;
     while ((long long)it * (it + 1) / 2 > t) --it;
     int jt = t - (int)((long long)it * (it + 1) / 2);
-    __shared__ double sx[64], sy[64], sz[64];   // column (j) points
-    int tid = threadIdx.x;
-    if (tid < 64) {
-        int j = jt * 64 + tid;
-        bool ok = j < n;
-        sx[tid] = ok ? ax[j] : 0.0;
-        sy[tid] = ok ? ay[j] : 0.0;
-        sz[tid] = (ok && KB_HASZ(DIM)) ? az[j] : 0.0;
-    }
-    __syncthreads();
-    int jl = tid & 63;          // column within tile (contiguous -> coalesced stores)
-    int i0 = tid >> 6;          // 0..3
-    int j = jt * 64 + jl;
-    for (int r = i0; r < 64; r += 4) {
-        int i = it * 64 + r;
-        double v;
-        if (i < n && j < n) {
-            if (i == j) v = vg.c0;
-            else {
-                double d = kb_dist<DIM>(ax[i], ay[i], KB_HASZ(DIM) ? az[i] : 0.0, sx[jl], sy[jl], sz[jl]);
-                v = vg.c0 - kb_gamma<MODEL>(vg, d);
-            }
-        } else {
-            v = (i == j) ? 1.0 : 0.0;
-        }
-        C[(size_t)i * ld + j] = v;
-    }
-}
-
-// the lower tiles of the tile rows [it0, n_pad / 64) only (kbk_append_factor: the new block row). The tile body is
-// assemble_kernel's, kept as its own copy so that the fresh assembly compiles exactly as before.
-template <int DIM, int MODEL>
-__global__ void __launch_bounds__(256) assemble_rows_kernel(VgParams vg, int n, int ld, int it0,
-                                                             const double* __restrict__ ax,
-                                                             const double* __restrict__ ay,
-                                                             const double* __restrict__ az,
-                                                             double* __restrict__ C) {
-    const int it = it0 + blockIdx.y, jt = blockIdx.x;
-    if (jt > it) return;
     __shared__ double sx[64], sy[64], sz[64];   // column (j) points
     int tid = threadIdx.x;
     if (tid < 64) {
@@ -458,15 +420,16 @@ __global__ void __launch_bounds__(128) syrk_kernel(double* __restrict__ C, int l
 
 // ---------------------------------------------------------------------------
 // K2b  triangular inverse by level doubling.  At level m (block size m = 64*2^s),
-// pair p covers rows [r0, r0+m) (top) and [r0+m, r0+m+m2) (bottom), r0 = 2*p*m:
+// pair p covers rows [r0, r0+m) (top) and [r0+m, r0+m+m2) (bottom), r0 = 2*p*m, m2 = min(mb, n_pad - r0 - m):
 //     W21 = -W22 * (L21 * W11)
 // step 1: T1 = L21 * W11   (W11 lower-triangular: k >= first column of the tile)
 // step 2: W21 = -W22 * T1  (W22 lower-triangular: k <= last row of the tile)
+// Level doubling passes mb = m; appended stations run one pair with the held rows on top (m = n0, mb = n_pad - n0).
 __global__ void __launch_bounds__(128) trtri_step1_kernel(const double* __restrict__ L, const double* __restrict__ W,
-                                                           double* __restrict__ T1, int ld, int n_pad, int m) {
+                                                           double* __restrict__ T1, int ld, int n_pad, int m, int mb) {
     __shared__ GemmSmem sm;
     int r0 = 2 * blockIdx.z * m;
-    int m2 = min(m, n_pad - r0 - m);
+    int m2 = min(mb, n_pad - r0 - m);
     int ti = blockIdx.y, tj = blockIdx.x;
     if (m2 <= 0 || ti * 64 >= m2) return;
     const double* A = L + (size_t)(r0 + m + ti * 64) * ld + r0;        // L21 rows
@@ -477,10 +440,10 @@ __global__ void __launch_bounds__(128) trtri_step1_kernel(const double* __restri
 }
 
 __global__ void __launch_bounds__(128) trtri_step2_kernel(double* __restrict__ W, const double* __restrict__ T1,
-                                                           int ld, int n_pad, int m) {
+                                                           int ld, int n_pad, int m, int mb) {
     __shared__ GemmSmem sm;
     int r0 = 2 * blockIdx.z * m;
-    int m2 = min(m, n_pad - r0 - m);
+    int m2 = min(mb, n_pad - r0 - m);
     int ti = blockIdx.y, tj = blockIdx.x;
     if (m2 <= 0 || ti * 64 >= m2) return;
     const double* A = W + (size_t)(r0 + m + ti * 64) * ld + (r0 + m);  // W22 rows of tile ti
@@ -505,29 +468,16 @@ __global__ void __launch_bounds__(128) gram_lower_kernel(const double* __restric
 }
 
 // ---------------------------------------------------------------------------
-// Appended stations (kb200_append_data, DESIGN.md §5g): the block row [n0, n_pad) of L and W from the held L11, W11 of
-// rows [0, n0). One 64x64 output tile (ti, tj) per CTA; the k range of each product skips the zero triangle of its
-// triangular factor:
-//   AP_L21   L21 = C21 W11^T        (NT)  W11[j][k] = 0 for k > j
-//   AP_SYRK  S   = C22 - L21 L21^T  (NT)  lower tiles only, k over [0, n0)
-//   AP_T     T   = L21 W11          (NN)  W11[k][j] = 0 for k < j
-//   AP_W21   W21 = -W22 T           (NN)  W22[i][k] = 0 for k > i
-// A, B and out point at the first row (and, for NN-B / out, column) of their blocks; all share the stride ld.
-enum AppendGemm { AP_L21 = 0, AP_SYRK = 1, AP_T = 2, AP_W21 = 3 };
-template <bool NT>
-__global__ void __launch_bounds__(128) append_gemm_kernel(const double* __restrict__ A, const double* __restrict__ B,
-                                                          double* __restrict__ out, int ld, int kend, int mode,
-                                                          double alpha, double beta) {
+// Appended stations (kb200_append_data, DESIGN.md §5g): L21 = C21 W11^T, the new rows [n0, n_pad) of L from the held
+// W11 of rows [0, n0). One 64x64 output tile (ti, tj) per CTA; W11[j][k] = 0 for k > j, so k stops at the end of the
+// column tile. C21 and L21 point at the first new row, column 0.
+__global__ void __launch_bounds__(128) append_l21_kernel(const double* __restrict__ C21, const double* __restrict__ W11,
+                                                         double* __restrict__ L21, int ld) {
     __shared__ GemmSmem sm;
     const int tj = blockIdx.x, ti = blockIdx.y;
-    int k0 = 0, k1 = kend;
-    if (mode == AP_L21) k1 = (tj + 1) * 64;
-    else if (mode == AP_SYRK) { if (tj > ti) return; }
-    else if (mode == AP_T) k0 = tj * 64;
-    else k1 = (ti + 1) * 64;
     double acc[4][4][2] = {};
-    gemm_tile_64<NT>(acc, sm, A + (size_t)ti * 64 * ld, ld, NT ? B + (size_t)tj * 64 * ld : B + tj * 64, ld, k0, k1);
-    gemm_tile_store(acc, out + (size_t)ti * 64 * ld + tj * 64, ld, alpha, beta);
+    gemm_tile_64<true>(acc, sm, C21 + (size_t)ti * 64 * ld, ld, W11 + (size_t)tj * 64 * ld, ld, 0, (tj + 1) * 64);
+    gemm_tile_store(acc, L21 + (size_t)ti * 64 * ld + tj * 64, ld, 1.0, 0.0);
 }
 
 // ---------------------------------------------------------------------------
@@ -710,12 +660,13 @@ cudaError_t kbk_adjust_data(int dim, const Aniso& an, int n, const double* x, co
     });
 }
 
-cudaError_t kbk_assemble(int dim, const VgParams& vg, int n, int n_pad, int ld,
+cudaError_t kbk_assemble(int dim, const VgParams& vg, int n, int n_pad, int ld, int it0,
                          const double* ax, const double* ay, const double* az, double* C, cudaStream_t st) {
     const int nb = n_pad / 64;
     return KbDims::dispatch(dim, [&](auto D) {
         return KbModels::dispatch(vg.model, [&](auto M) {
-            assemble_kernel<D, M><<<nb * (nb + 1) / 2, 256, 0, st>>>(vg, n, n_pad, ld, ax, ay, az, C);
+            const int tiles = nb * (nb + 1) / 2 - it0 * (it0 + 1) / 2;
+            assemble_kernel<D, M><<<tiles, 256, 0, st>>>(vg, n, ld, it0, ax, ay, az, C);
             return cudaGetLastError();
         });
     });
@@ -734,9 +685,9 @@ cudaError_t kbk_factor_init() {
 // the high-priority stream `hi` UNDER the DMMA-bound trailing update of the previous panel. Events (ev[0..2*nob)) order
 // the read-modify-write passes over shared regions:
 //   T_look(ob) after T_rest(ob-1);  T_rest(ob) after panel(ob).
-// The diagonal-block inverses land in W's diagonal blocks (input of kbk_trtri).
-cudaError_t kbk_cholesky(double* C, double* W, double* Lstage, int ld, int n_pad, int* flag, double dtol, cudaStream_t st,
-                         cudaStream_t hi, cudaEvent_t* ev, int n_ev, int* launches) {
+// The diagonal-block inverses land in W's diagonal blocks (input of kbk_inverse_rows).
+static cudaError_t cholesky(double* C, double* W, double* Lstage, int ld, int n_pad, int* flag, double dtol, cudaStream_t st,
+                            cudaStream_t hi, cudaEvent_t* ev, int n_ev, int* launches) {
     const int nb = n_pad / 64;
     const int OW = 4;
     const int nob = (nb + OW - 1) / OW;
@@ -776,49 +727,40 @@ cudaError_t kbk_cholesky(double* C, double* W, double* Lstage, int ld, int n_pad
     return cudaGetLastError();
 }
 
-cudaError_t kbk_trtri(const double* L, double* W, double* T1, int ld, int n_pad, cudaStream_t st, int* launches) {
-    for (int m = 64; m < n_pad; m *= 2) {
-        int pairs = (n_pad + 2 * m - 1) / (2 * m);
-        dim3 grid(m / 64, m / 64, pairs);
-        trtri_step1_kernel<<<grid, 128, 0, st>>>(L, W, T1, ld, n_pad, m);
-        trtri_step2_kernel<<<grid, 128, 0, st>>>(W, T1, ld, n_pad, m);
-        *launches += 2;
-    }
-    return cudaGetLastError();
-}
-
-cudaError_t kbk_assemble_rows(int dim, const VgParams& vg, int n, int n_pad, int ld, int it0,
-                              const double* ax, const double* ay, const double* az, double* C, cudaStream_t st) {
-    const int nb = n_pad / 64;
-    return KbDims::dispatch(dim, [&](auto D) {
-        return KbModels::dispatch(vg.model, [&](auto M) {
-            assemble_rows_kernel<D, M><<<dim3(nb, nb - it0), 256, 0, st>>>(vg, n, ld, it0, ax, ay, az, C);
-            return cudaGetLastError();
-        });
-    });
-}
-
-// L21 = C21 W11^T, S = C22 - L21 L21^T, L22 = chol(S), W22 = L22^-1 (the panel chain and level-doubling inverse of a
-// fresh factorisation, on the corner), W21 = -W22 (L21 W11). T is scratch of C's shape: L21 waits there until the Schur
-// complement has read it, then the corner's staged diagonal factors and T1 of the inverse, then T = L21 W11.
-cudaError_t kbk_append_factor(double* C, double* W, double* T, int ld, int n_pad, int n0, int* flag, double dtol,
+// Rows [n0, n_pad) of L and W from the held L11 (in C) and W11 = L11^-1 of rows [0, n0); n0 = 0 factors all of C:
+//   kbk_cholesky_rows  L21 = C21 W11^T, S = C22 - L21 L21^T, L22 = chol(S)      (the Cholesky above, on the corner)
+//   kbk_inverse_rows   W22 = L22^-1 (level doubling on the corner), W21 = -W22 (L21 W11): one more doubling step whose
+//                      top block is the n0 held rows
+// T is scratch of C's shape. L21 goes there first (its tiles read whole rows of C21), then into C21 for the Schur
+// update; afterwards T holds the corner's staged diagonal factors, then T1 of the inverse.
+cudaError_t kbk_cholesky_rows(double* C, double* W, double* T, int ld, int n_pad, int n0, int* flag, double dtol,
                               cudaStream_t st, cudaStream_t hi, cudaEvent_t* ev, int n_ev, int* launches) {
-    const int nb0 = n0 / 64, nbr = (n_pad - n0) / 64;
+    const int nb0 = n0 / 64, nb = n_pad / 64;
     const size_t r0 = (size_t)n0 * ld;
-    double* C22 = C + r0 + n0;
-    double* W22 = W + r0 + n0;
     if (nb0 > 0) {
-        append_gemm_kernel<true><<<dim3(nb0, nbr), 128, 0, st>>>(C + r0, W, T + r0, ld, n0, AP_L21, 1.0, 0.0);
-        append_gemm_kernel<true><<<dim3(nbr, nbr), 128, 0, st>>>(T + r0, T + r0, C22, ld, n0, AP_SYRK, -1.0, 1.0);
+        append_l21_kernel<<<dim3(nb0, nb - nb0), 128, 0, st>>>(C + r0, W, T + r0, ld);
         KB_CUDA_OK(cudaMemcpy2DAsync(C + r0, (size_t)ld * 8, T + r0, (size_t)ld * 8, (size_t)n0 * 8, n_pad - n0,
                                      cudaMemcpyDeviceToDevice, st));
+        syrk_kernel<<<dim3(nb - nb0, nb - nb0), 128, 0, st>>>(C, ld, 0, nb0, nb0, nb);
         *launches += 2;
     }
-    KB_CUDA_OK(kbk_cholesky(C22, W22, T, ld, n_pad - n0, flag, dtol, st, hi, ev, n_ev, launches));
-    KB_CUDA_OK(kbk_trtri(C22, W22, T + r0 + n0, ld, n_pad - n0, st, launches));
-    if (nb0 > 0) {
-        append_gemm_kernel<false><<<dim3(nb0, nbr), 128, 0, st>>>(C + r0, W, T + r0, ld, n0, AP_T, 1.0, 0.0);
-        append_gemm_kernel<false><<<dim3(nb0, nbr), 128, 0, st>>>(W22, T + r0, W + r0, ld, 0, AP_W21, -1.0, 0.0);
+    return cholesky(C + r0 + n0, W + r0 + n0, T, ld, n_pad - n0, flag, dtol, st, hi, ev, n_ev, launches);
+}
+
+cudaError_t kbk_inverse_rows(const double* L, double* W, double* T, int ld, int n_pad, int n0, cudaStream_t st,
+                             int* launches) {
+    const size_t c0 = (size_t)n0 * ld + n0;
+    const int nc = n_pad - n0;
+    for (int m = 64; m < nc; m *= 2) {
+        dim3 grid(m / 64, m / 64, (nc + 2 * m - 1) / (2 * m));
+        trtri_step1_kernel<<<grid, 128, 0, st>>>(L + c0, W + c0, T + c0, ld, nc, m, m);
+        trtri_step2_kernel<<<grid, 128, 0, st>>>(W + c0, T + c0, ld, nc, m, m);
+        *launches += 2;
+    }
+    if (n0 > 0) {
+        dim3 grid(n0 / 64, nc / 64, 1);
+        trtri_step1_kernel<<<grid, 128, 0, st>>>(L, W, T, ld, n_pad, n0, nc);
+        trtri_step2_kernel<<<grid, 128, 0, st>>>(W, T, ld, n_pad, n0, nc);
         *launches += 2;
     }
     return cudaGetLastError();

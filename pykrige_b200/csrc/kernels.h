@@ -208,18 +208,16 @@ __device__ __forceinline__ void kb_finalize_point(const SolvePtParams& P, long l
 
 cudaError_t kbk_adjust_data(int dim, const Aniso& an, int n, const double* x, const double* y, const double* z,
                             double* ax, double* ay, double* az, cudaStream_t st);
-cudaError_t kbk_assemble(int dim, const VgParams& vg, int n, int n_pad, int ld,
+// C = c0 11^T - Gamma: the lower tiles of the tile rows [it0, n_pad / 64)
+cudaError_t kbk_assemble(int dim, const VgParams& vg, int n, int n_pad, int ld, int it0,
                          const double* ax, const double* ay, const double* az, double* C, cudaStream_t st);
-cudaError_t kbk_cholesky(double* C, double* W, double* Lstage, int ld, int n_pad, int* flag, double dtol, cudaStream_t st,
-                         cudaStream_t hi, cudaEvent_t* ev, int n_ev, int* launches);   // Lstage: (n_pad/64) x 4096 doubles of scratch;
-                                                                                       // hi: high-priority side stream; ev: >= 2*ceil(n_pad/256)+1 events
-cudaError_t kbk_trtri(const double* L, double* W, double* T1, int ld, int n_pad, cudaStream_t st, int* launches);
-// appended stations (DESIGN.md §5g): C rows [it0 * 64, n_pad), lower tiles; then the block row [n0, n_pad) of L (in C)
-// and W from L11, W11 of rows [0, n0) (n0 a multiple of 64). T: scratch of C's shape; flag as kbk_cholesky (column - n0)
-cudaError_t kbk_assemble_rows(int dim, const VgParams& vg, int n, int n_pad, int ld, int it0,
-                              const double* ax, const double* ay, const double* az, double* C, cudaStream_t st);
-cudaError_t kbk_append_factor(double* C, double* W, double* T, int ld, int n_pad, int n0, int* flag, double dtol,
+// Rows [n0, n_pad) of L (in C) and W = L^-1 from the held rows [0, n0) (n0 a multiple of 64; n0 = 0: all of C).
+// kbk_cholesky_rows leaves a non-positive pivot in *flag as 1 + its column - n0; kbk_inverse_rows runs after it
+// succeeded. T: scratch of C's shape; hi: high-priority side stream; ev: >= 2*ceil((n_pad - n0)/256)+1 events
+cudaError_t kbk_cholesky_rows(double* C, double* W, double* T, int ld, int n_pad, int n0, int* flag, double dtol,
                               cudaStream_t st, cudaStream_t hi, cudaEvent_t* ev, int n_ev, int* launches);
+cudaError_t kbk_inverse_rows(const double* L, double* W, double* T, int ld, int n_pad, int n0, cudaStream_t st,
+                             int* launches);
 // nv value columns (column-major, stride n): Fz / Hz / Uz hold K + 1 + nv columns of stride n_pad each
 cudaError_t kbk_dual(const double* W, int ld, int n, int n_pad, int n_rl, int n_hd, int nv,
                      const double* ax, const double* ay, const double* az, const DriftScale& ds,
